@@ -1,5 +1,5 @@
 /*
- * rz_engine.h -- C ABI of librz_engine.so: the B200-native self-play hot path of reversi-alpha-zero.
+ * rz_engine.h -- C ABI of librz_engine.so: the H100-native self-play hot path of reversi-alpha-zero.
  *
  * The reference (mokemokechicken/reversi-alpha-zero) has no FFI seam: its self-play path is Python
  * calling Python (SURVEY.md section 8(b)).  Each entry point below therefore names the reference
@@ -110,15 +110,14 @@ typedef struct rz_net_cfg {
     int32_t kernel_size; /* ModelConfig.cnn_filter_size  (config.py:190); only 3 is supported */
 } rz_net_cfg;
 
-#define RZ_NET_IMPL_AUTO 0    /* tcgen05 tower when filters == 256, else the generic kernel */
+#define RZ_NET_IMPL_AUTO 0    /* wgmma tower when filters == 256, else the generic kernel */
 #define RZ_NET_IMPL_GENERIC 1 /* CUDA-core fp32 kernel, any configuration */
-#define RZ_NET_IMPL_TCGEN05 2 /* fused persistent tcgen05 tower (filters must be 256) */
+#define RZ_NET_IMPL_TCGEN05 2 /* fused persistent tensor-core (wgmma) tower (filters must be 256) */
 
-/* Which kernel serves RZ_NET_IMPL_TCGEN05 from now on (process-wide): 1 = one CTA per tile (csrc/rz_net_tc.cu),
- * 2 = CTA pairs, cta_group::2, epilogue overlapped with the MMA stream (csrc/rz_net_tc2.cu).  The default comes from
- * the environment variable RZ_TOWER_KERNEL when the first network call is made (default 2).  Used by the tests and benchmarks to
- * run both on the same inputs. */
-int rz_net_set_tower_kernel(int version);
+/* Thread-block clusters of the tensor-core tower from now on (process-wide): 2 = CTA pairs that share every weight stage
+ * through cluster multicast (default; falls back to 1 where the GPU cannot hold a pair), 1 = single CTAs.  The default
+ * comes from the environment variable RZ_TOWER_CLUSTER when the first network call is made. */
+int rz_net_set_tower_cluster(int cluster);
 int rz_net_create(const rz_net_cfg* cfg, int device, rz_net** out);
 int rz_net_destroy(rz_net* net);
 /* number of float32 values in the weight blob for this configuration.  Blob layout (Keras tensor
@@ -136,7 +135,7 @@ int rz_net_load_weights_dev(rz_net* net, const float* blob_dev, size_t n_floats,
  * policy[n][64] softmax probabilities, value[n] tanh.  Device pointers. */
 int rz_net_predict_dev(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value,
                        size_t n, int impl, void* stream);
-/* diagnostic variant of the tcgen05 path: additionally writes the fp32 residual-tower output
+/* diagnostic variant of the tensor-core tower path: additionally writes the fp32 residual-tower output
  * tower[n][64 pixels][256 channels] (pixel = y*8+x) so tests can localise a numerical difference. */
 int rz_net_debug_tower_dev(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value,
                            float* tower, size_t n, void* stream);

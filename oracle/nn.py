@@ -55,7 +55,7 @@ def _fold(w, name):
 
 @torch.no_grad()
 def forward_fp16_operands(w, planes, n_res, round_weights=True, round_acts=True):
-    """The SAME network evaluated the way the tcgen05 tower is specified to evaluate it: convolution operands rounded
+    """The SAME network evaluated the way the tensor-core tower is specified to evaluate it: convolution operands rounded
     to fp16 (round-to-nearest-even; weights of all 1 + 2R convolutions, activations of the 2R tower convolutions -- the
     first layer's {0,1} planes are exact), products and sums exact (fp64 here; the tensor core accumulates in fp32),
     folded BatchNorm / residual stream / heads in fp32.  The difference between this and `forward` is the error the

@@ -34,8 +34,9 @@ namespace solver {
 constexpr int kBlockThreads = 128;
 // The engine's solver step: advance every unfinished request of a slot group for at most `budget_ns`, then queue what is
 // still unfinished for the group's next wave.  `active` holds request-context indices: the unfinished ones of the last
-// wave followed by those the tick kernel just added.  One CTA per SM, so all of them are resident beside the other
-// group's network kernel and the step costs at most about `budget_ns` of stream time.
+// wave followed by those the tick kernel just added.  One CTA per SM.  A CTA of the tower kernel takes nearly all of an
+// SM's registers, so these CTAs start only on SMs the other group's tower launch leaves free or after it ends; the budget
+// bounds the time a CTA runs once it has started, not the stream time of the step.
 __global__ void __launch_bounds__(kBlockThreads) solve_active_kernel(SolveCtx* __restrict__ ctx, const uint32_t* __restrict__ active,
                                                                      const uint32_t* __restrict__ n_active, uint32_t* __restrict__ next,
                                                                      uint32_t* __restrict__ n_next, u64* tt_base, long long budget_ns) {
@@ -333,7 +334,7 @@ static int launch_wave(rz_engine* e) {
         tick_warp_kernel<<<(s1 - s0 + 1) / 2, kWarpTickThreads, 0, st>>>(c, e->dp, s0, s1, g, par);
         RZ_LAUNCH_CHECK();
         e->mcts_launches++;
-        if (solving) {  // advance the group's unfinished solves for a bounded time (underneath the other group's tower)
+        if (solving) {  // advance the group's unfinished solves for a bounded time (on the SMs the other group's tower leaves free)
             const size_t list = (size_t)c.G * (c.K + 1);
             solver::solve_active_kernel<<<num_sms(), solver::kBlockThreads, 0, st>>>(
                 e->dp.sctx, e->dp.sactive + (g * 2 + par) * list, e->dp.solve_count + (g * 2 + par) * 64,
@@ -403,7 +404,8 @@ int rz_engine_create(const rz_engine_cfg* cfg, rz_net* net, int device, rz_engin
     e->ev_used = 0; e->nn_ms = e->mcts_ms = e->run_ms = 0.0;
     for (int i = 0; i < 48; ++i) e->ev[i] = nullptr;
     e->ev_run[0] = e->ev_run[1] = e->ev_run[2] = nullptr;
-    // two slot groups on two streams: the MCTS tick of one group runs underneath the network launch of the other
+    // two slot groups on two streams: the MCTS tick of one group can run while the network launch of the other is in flight,
+    // on the SMs that launch leaves free (a tower CTA takes nearly all of an SM's registers), or right after it
     e->n_groups = cfg->overlap_groups == 1 ? 1 : (cfg->overlap_groups == 2 ? 2 : (cfg->games >= 256 ? 2 : 1));
     if (cfg->games < 2) e->n_groups = 1;
     e->group_slot0[0] = 0;

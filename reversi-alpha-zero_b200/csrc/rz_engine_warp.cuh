@@ -614,7 +614,7 @@ struct WCtx {
     }
 };
 
-constexpr int kWarpTickThreads = 64;  // 2 game slots per CTA: 64 x 124 registers fit beside a resident tower CTA (320 x 168)
+constexpr int kWarpTickThreads = 64;  // 2 game slots per CTA
 
 __global__ void __launch_bounds__(kWarpTickThreads) tick_warp_kernel(const DevCfg c, const DevPtrs p, const int slot0, const int slot_end,
                                                                      const int group, const int parity) {

@@ -21,18 +21,21 @@ struct rz_net {
     size_t off_conv0, off_res0, res_stride_conv;  // kernel offset of conv0; of res0.conv1; floats per (conv+bn) group
     size_t off_policy_conv, off_policy_fc_k, off_policy_fc_b;
     size_t off_value_conv, off_value_fc1_k, off_value_fc1_b, off_value_fc2_k, off_value_fc2_b;
-    // tcgen05 tower (F == 256 only)
-    __half* tc_w0;       // [4 kc][256 n][8] fp16: layer-0 weights, K = 18 padded to 32, UMMA K-major no-swizzle image
+    // wgmma tower (F == 256 only)
+    __half* tc_w0;       // [4 kc][256 n][8] fp16: layer-0 weights, K = 18 padded to 32, K-major no-swizzle image
     __half* tc_w;        // [2R layers][36 stages][8 kc][256 n][8] fp16: one 32 KB shared-memory image per pipeline stage
-    // pair kernel (rz_net_tc2.cu, cta_group::2): the same weights in the order its K / N loops consume them
-    __half* tc2_w0;      // [cta 2][nh 2][kc 4][n 64][8]
-    __half* tc2_w;       // [2R layers][36 stages][cta 2][kbl 2][kc 8][n 64][8]: one 16 KB image per CTA and pipeline stage
+    // fp32 residual-stream scratch of the tower kernel ([CTA][kTowerResFloatsPerCta]); launches from different streams
+    // are ordered through res_done, recorded after every launch that uses it
+    float* res;
+    cudaEvent_t res_done;
     // scratch for the host-buffer predict path
     void* scratch;
     size_t scratch_bytes;
 };
 
 namespace rz {
+
+constexpr size_t kTowerResFloatsPerCta = 256 * 128;  // 128 KB: 256 math threads x 128 fp32 accumulators
 
 inline int n_conv_layers(const rz_net_cfg& c) { return 1 + 2 * c.res_blocks; }
 // per-layer folded BN parameters: scale at [l][0][*], shift at [l][1][*]
@@ -48,14 +51,8 @@ int net_forward_tc(rz_net* net, const uint64_t* own, const uint64_t* enemy, floa
                    const uint32_t* n_dev = nullptr /* nullable: actual batch size in device memory (<= n) */,
                    float* dbg_logits = nullptr /* nullable: [n][64] policy logits */, float* dbg_vlogit = nullptr /* nullable: [n] */);
 int net_pack_tc(rz_net* net, cudaStream_t stream);
-// the CTA-pair kernel (rz_net_tc2.cu); same contract as net_forward_tc
-int net_forward_tc2(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value, size_t n,
-                    cudaStream_t stream, float* dbg_tower, const uint32_t* n_dev = nullptr, float* dbg_logits = nullptr,
-                    float* dbg_vlogit = nullptr);
-int net_pack_tc2(rz_net* net, cudaStream_t stream);
-// which tcgen05 tower kernel serves RZ_NET_IMPL_TCGEN05: 2 = CTA pairs with overlapped epilogue (default), 1 = one CTA per
-// tile (RZ_TOWER_KERNEL=1, rz_net_set_tower_kernel)
-int tower_kernel_version();
+// thread-block clusters of the tower kernel: 2 = CTA pairs sharing the weight stages (default), 1 = single CTAs
+int set_tower_cluster(int cluster);
 int net_forward(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value, size_t n, int impl,
                 cudaStream_t stream);
 

@@ -1,27 +1,31 @@
-// rz_net_tc.cu -- K4/K5: fused persistent tcgen05 residual tower + heads for the 256-filter network.
+// rz_net_tc.cu -- K4/K5: fused persistent wgmma residual tower + heads for the 256-filter network (sm_90a).
 //
 // One CTA per SM, each CTA owns a tile of TWO boards (M = 128 pixel rows) and carries it through the
-// WHOLE network without touching HBM in between:
-//   * activations live in shared memory as fp16 in the UMMA "K-major, no-swizzle" canonical layout,
+// WHOLE network without writing activations to HBM in between:
+//   * activations live in shared memory as fp16 in the wgmma "K-major, no-swizzle" canonical layout,
 //     with a one-pixel zero border, so that each of the nine 3x3 taps is just a different start
 //     address of the same buffer (implicit GEMM, no im2col copy):
 //         chunk(cg, slot, xp) at cg*2896 + slot*144 + xp*16 bytes   (8 channels = 16 B per chunk)
 //         slot = 2*(y+1) + board (the two boards' rows are interleaved so that a dy shift is a
 //         uniform 2-slot offset), xp = x+1; xp = 9 of one slot aliases xp = 0 of the next (shared
 //         zero chunk).  MMA row m = (2y+board)*8 + x  ->  8-row core matrices are board rows.
-//   * weights (fp16, 1.18 MB per conv, L2-resident) are streamed by a producer thread with
+//   * weights (fp16, 1.18 MB per conv, L2-resident) are streamed by a producer warp with
 //     cp.async.bulk in pre-packed 32 KB stages (one tap x 64 input channels x 256 output channels)
-//     through a 3-deep mbarrier ring;
-//   * one thread issues tcgen05.mma (M=128, N=256, K=16, fp16 in / fp32 accumulate): 144 MMAs per conv
-//     layer into a 256-column TMEM accumulator;
-//   * eight epilogue warps read the accumulator with tcgen05.ld, apply the folded BatchNorm
-//     (scale, shift), the residual (kept in fp32 in the other 256 TMEM columns) and ReLU, and write the
-//     next layer's fp16 activations straight back into the shared-memory operand buffer;
+//     through a 3-deep mbarrier ring; with clusters of two CTAs each CTA fetches half of every stage
+//     and multicasts it into both CTAs' shared memory, which halves the L2 -> SM weight traffic;
+//   * two math warpgroups, one per 64 rows (the rows y = 0-3 / 4-7 of both boards), issue
+//     wgmma.m64n256k16 (fp16 in / fp32 accumulate in registers): 144 per conv layer and warpgroup;
+//   * the same warpgroups then apply the folded BatchNorm (scale, shift), the skip connection and
+//     ReLU to their accumulators and write the next layer's fp16 activations straight back into the
+//     shared-memory operand buffer.  The fp32 residual stream (the block inputs) does not fit beside
+//     the accumulators in the register file, nor beside the operands in shared memory; it goes to a
+//     per-CTA global scratch of the network (128 KB, written once and read once per block, L2-resident);
 //   * the first conv (2 -> 256 channels, K = 18 padded to 32) is a 2-MMA GEMM on an im2col tile built
-//     from the two bitboards; the policy / value heads run on the epilogue warps from the fp32 tower
+//     from the two bitboards; the policy / value heads run on the math warps from the fp32 tower
 //     output.
 // HBM traffic per position: 16 B in, 260 B out.  Algorithmic work: 2 * 755,343,616 flop (SURVEY 3.2).
 #include <stdlib.h>
+#include <mutex>
 #include "rz_bitboard.cuh"
 #include "rz_net.cuh"
 #include "rz_tc_common.cuh"
@@ -29,8 +33,12 @@
 namespace rz {
 namespace tc {
 
-constexpr int kThreads = 320;  // warp 0 producer, warp 1 MMA issuer + TMEM owner, warps 2..9 epilogue
-constexpr int kEpiThreads = 256;
+// warps 0..7 = two math warpgroups, warps 8..11 = producer warpgroup (one thread streams the weights).  Registers are
+// handed from the producer warpgroup to the math warpgroups (setmaxnreg): the math threads hold a 64 x 256 fp32
+// accumulator (128 registers) each.
+constexpr int kThreads = 384;
+constexpr uint32_t kProducerRegs = 40, kMathRegs = 232;
+constexpr int kMathThreads = 256;
 constexpr uint32_t kActCg = 2896, kActSlot = 144;
 constexpr uint32_t kActBytes = 32 * kActCg;  // 92,672
 constexpr uint32_t kStageBytes = 32768, kStages = 3;
@@ -44,28 +52,18 @@ constexpr uint32_t kOffPart = kOffSS + 2 * 2048;         // [2 halves][128 rows]
 constexpr uint32_t kOffHp = kOffPart + 2 * 128 * 4 * 4;  // [2 boards][128]
 constexpr uint32_t kOffHv = kOffHp + 2 * 128 * 4;        // [2][64]
 constexpr uint32_t kOffLogit = kOffHv + 2 * 64 * 4;      // [2][64]
-constexpr uint32_t kMaxV = 512;
-constexpr uint32_t kOffFc1 = kOffLogit + 2 * 64 * 4;     // [2][kMaxV]
-constexpr uint32_t kOffBar = kOffFc1 + 2 * kMaxV * 4;    // mbarriers
-constexpr uint32_t kNumBars = 2 * kStages + 3;
-constexpr uint32_t kOffTmemPtr = kOffBar + kNumBars * 8;
-constexpr uint32_t kSmemBytes = kOffTmemPtr + 16;
+constexpr uint32_t kOffFc1 = kOffLogit + 2 * 64 * 4;     // [2][kTcMaxV]
+constexpr uint32_t kOffBar = kOffFc1 + 2 * kTcMaxV * 4;  // mbarriers
+constexpr uint32_t kNumBars = 2 * kStages + 1;           // full[], empty[], w0
+constexpr uint32_t kSmemBytes = kOffBar + kNumBars * 8;
 constexpr uint32_t kSmemAlloc = kSmemBytes + 128;  // slack for manual 128 B alignment
 static_assert(kSmemAlloc <= 232448, "shared memory budget exceeded");
-
-// instruction descriptor, kind::f16: D = f32 (bits 4-5 = 1), A = B = f16 (0), K-major both,
-// N >> 3 at bits 17-22, M >> 4 at bits 24-28
-constexpr uint32_t kIdesc = (1u << 4) | ((256u >> 3) << 17) | ((128u >> 4) << 24);
+static_assert(kTowerResFloatsPerCta == (size_t)kMathThreads * 128, "residual scratch per CTA");
 
 // CL = thread-block-cluster size (1 or 2).  With CL = 2 the two CTAs of a cluster each fetch half of every weight
-// stage from L2 and multicast it into both CTAs' shared memory (L2 -> SM weight traffic halves); MMAs, TMEM and the
-// epilogue stay per-CTA (cta_group::1).  A stage may be refilled only after BOTH CTAs' MMAs have read it, so the
-// `empty` barriers count CL commits (each MMA thread commits to every CTA of the cluster).
-// EXP != 0 are MEASUREMENT variants (RZ_TOWER_EXPERIMENT, tools/nn_bench.py; results are garbage): 1 = the epilogue only
-// keeps the barrier protocol (no accumulator read-out, no BN / ReLU, no operand stores): the time of the MMA stream alone,
-// i.e. what a perfect overlap of epilogue and MMA could reach; 2 = the MMA thread issues no MMAs (barriers only): the time
-// of the epilogues alone.
-template <int CL, int EXP = 0>
+// stage from L2 and multicast it into both CTAs' shared memory; MMAs and the epilogue stay per-CTA.  A stage may be
+// refilled only after BOTH CTAs' math warps have read it, so the `empty` barriers count the arrivals of 8 warps per CTA.
+template <int CL>
 __global__ void __launch_bounds__(kThreads, 1) net_tower_kernel(const Params pp) {
     Params p = pp;
     if (p.n_dev) p.n = *p.n_dev;
@@ -76,42 +74,34 @@ __global__ void __launch_bounds__(kThreads, 1) net_tower_kernel(const Params pp)
     const uint32_t bar0 = base + kOffBar;
     auto bar_full = [&](uint32_t s) { return bar0 + s * 8; };
     auto bar_empty = [&](uint32_t s) { return bar0 + (kStages + s) * 8; };
-    const uint32_t bar_w0 = bar0 + 2 * kStages * 8, bar_a = bar_w0 + 8, bar_acc = bar_w0 + 16;
+    const uint32_t bar_w0 = bar0 + 2 * kStages * 8;
     const uint32_t ntiles = (p.n + 1) >> 1;
     const int L = p.n_layers;
-    // every CTA of a cluster runs the same number of tile iterations (the producers / MMA threads are coupled through
-    // the shared weight ring); a CTA whose last tile index is past the batch processes an all-empty dummy tile
+    // every CTA of a cluster runs the same number of tile iterations (the producers are coupled through the shared
+    // weight ring); a CTA whose last tile index is past the batch processes an all-empty dummy tile
     const uint32_t crank = CL > 1 ? cluster_ctarank() : 0u;
     const uint32_t cbase = blockIdx.x - crank;
     const uint32_t iters = cbase < ntiles ? (ntiles - cbase + gridDim.x - 1) / gridDim.x : 0u;
-    constexpr uint16_t kMask = (uint16_t)((1u << CL) - 1u);
 
     // ---- one-time setup -----------------------------------------------------------------------------
     for (uint32_t i = threadIdx.x * 16; i < kActBytes; i += kThreads * 16) *reinterpret_cast<uint4*>(sm + kOffAct + i) = make_uint4(0, 0, 0, 0);
     fence_proxy_async();
     if (threadIdx.x == 0) {
-        for (uint32_t s = 0; s < kStages; ++s) { mbar_init(bar_full(s), 1); mbar_init(bar_empty(s), CL); }
+        for (uint32_t s = 0; s < kStages; ++s) { mbar_init(bar_full(s), 1); mbar_init(bar_empty(s), 8 * CL); }
         mbar_init(bar_w0, 1);
-        mbar_init(bar_a, kEpiThreads);
-        mbar_init(bar_acc, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {  // TMEM: all 512 columns (this kernel is the only resident CTA on its SM)
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(base + kOffTmemPtr) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
     if (CL > 1) cluster_sync_all();  // peers' barriers are initialised before anyone multicasts into them
-    tc_fence_after();
-    const uint32_t tmem = *reinterpret_cast<volatile uint32_t*>(sm + kOffTmemPtr);
-    const uint32_t tm_acc = tmem, tm_res = tmem + 256;
 
-    if (warp == 0) {
+    if (warp >= 8) {
         // ===== weight producer =====================================================================
-        if (lane == 0) {
-            mbar_expect_tx(bar_w0, kW0Bytes);
-            bulk_g2s(base + kOffW0, p.w0, kW0Bytes, bar_w0);
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProducerRegs));
+        if (warp == 8 && lane == 0) {
+            if (iters > 0) {   // a CTA without tiles must not leave with a copy into its shared memory in flight
+                mbar_expect_tx(bar_w0, kW0Bytes);
+                bulk_g2s(base + kOffW0, p.w0, kW0Bytes, bar_w0);
+            }
             uint32_t stage = 0, phase = 0;
             for (uint32_t it = 0; it < iters; ++it) {
                 for (int l = 1; l < L; ++l) {
@@ -124,143 +114,161 @@ __global__ void __launch_bounds__(kThreads, 1) net_tower_kernel(const Params pp)
                         } else {  // this CTA's slice of the stage, delivered to every CTA of the cluster
                             constexpr uint32_t kSlice = kStageBytes / CL;
                             bulk_g2s_mc(base + kOffW + stage * kStageBytes + crank * kSlice, src + (size_t)s * kStageBytes + crank * kSlice,
-                                        kSlice, bar_full(stage), kMask);
+                                        kSlice, bar_full(stage), (uint16_t)((1u << CL) - 1u));
                         }
                         if (++stage == kStages) { stage = 0; phase ^= 1; }
                     }
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer ==========================================================================
-        if (lane == 0) {
-            uint32_t stage = 0, phase = 0, a_par = 0;
-            bool first = true;
-            for (uint32_t it = 0; it < iters; ++it) {
-                for (int l = 0; l < L; ++l) {
-                    mbar_wait(bar_a, a_par);
-                    a_par ^= 1;
-                    tc_fence_after();
-                    if (l == 0) {
-                        if (first) { mbar_wait(bar_w0, 0); first = false; }
-#pragma unroll
-                        for (uint32_t j = 0; j < 2; ++j)
-                            umma_f16(tm_acc, smem_desc(base + kOffA0 + j * 2 * 2048, 2048, 128),
-                                     smem_desc(base + kOffW0 + j * 2 * 4096, 4096, 128), kIdesc, j);
-                    } else {
-                        for (uint32_t tap = 0; tap < 9; ++tap) {
-                            // tap (kh, kw) reads input pixel (y + kh - 1, x + kw - 1): slot offset 2*kh, chunk offset kw
-                            const uint32_t a_tap = base + kOffAct + (2 * (tap / 3)) * kActSlot + (tap % 3) * 16;
-                            for (uint32_t kb = 0; kb < 4; ++kb) {
-                                mbar_wait(bar_full(stage), phase);
-                                tc_fence_after();
-                                const uint32_t b_st = base + kOffW + stage * kStageBytes;
-                                if (EXP != 2) {
-#pragma unroll
-                                    for (uint32_t j = 0; j < 4; ++j)
-                                        umma_f16(tm_acc, smem_desc(a_tap + (kb * 8 + 2 * j) * kActCg, kActCg, kActSlot),
-                                                 smem_desc(b_st + 2 * j * 4096, 4096, 128), kIdesc, (tap | kb | j) != 0);
-                                }
-                                if (CL == 1) umma_commit(bar_empty(stage)); else umma_commit_mc(bar_empty(stage), kMask);
-                                if (++stage == kStages) { stage = 0; phase ^= 1; }
-                            }
-                        }
-                    }
-                    umma_commit(bar_acc);
-                }
-            }
-        }
     } else {
-        // ===== epilogue warps (8) ==================================================================
-        const int et = threadIdx.x - 64;        // 0..255
-        const int q = warp & 3;                 // TMEM sub-partition this warp may access
-        const int h = (warp - 2) >> 2;          // column half handled by this warp
-        const int m = q * 32 + lane;            // accumulator row == TMEM lane
-        const int g = m >> 3, x = m & 7, brd = g & 1, y = g >> 1;
-        const uint32_t lane_sel = (uint32_t)(q * 32) << 16;
+        // ===== math warpgroups (2) =================================================================
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kMathRegs));
+        const int et = threadIdx.x;           // 0..255
+        const int wg = warp >> 2;             // rows wg*64 .. wg*64 + 63
+        // accumulator fragment of wgmma m64n256: d[4i + 0/1] = row r0, columns c, c + 1; d[4i + 2/3] = row r0 + 8;
+        // c = 8i + 2 (lane & 3).  Rows r0 and r0 + 8 are the same pixel (y, x) of board 0 and board 1.
+        const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+        const int g0 = r0 >> 3, x = r0 & 7, y = g0 >> 1;
+        const int cq = 2 * (lane & 3);
+        const uint32_t act_row0 = base + kOffAct + (g0 + 2) * kActSlot + (x + 1) * 16 + cq * 2;  // + cg * kActCg
+        const uint32_t act_row1 = act_row0 + kActSlot;
+        const uint32_t a_wg = base + kOffAct + wg * 8 * kActSlot;   // operand rows of this warpgroup, tap (0, 0)
         float* ss_s = reinterpret_cast<float*>(sm + kOffSS);
         float* part = reinterpret_cast<float*>(sm + kOffPart);
         float* hp = reinterpret_cast<float*>(sm + kOffHp);
         float* hv = reinterpret_cast<float*>(sm + kOffHv);
         float* logit = reinterpret_cast<float*>(sm + kOffLogit);
         float* fc1 = reinterpret_cast<float*>(sm + kOffFc1);
-        const uint32_t act_row = base + kOffAct + (g + 2) * kActSlot + (x + 1) * 16;  // + cg * kActCg
-        uint32_t acc_par = 0;
-        uint32_t ss_buf = 0;
+        float4* res = reinterpret_cast<float4*>(p.res + (size_t)blockIdx.x * kTowerResFloatsPerCta) + et;   // + i * 256
+        const float* wpc = p.blob + p.off_policy_conv;
+        const float* wvc = p.blob + p.off_value_conv;
+        uint32_t stage = 0, phase = 0, ss_buf = 0;
+        float d[128];
 
         for (uint32_t it = 0; it < iters; ++it) {
             const uint32_t tile = blockIdx.x + it * gridDim.x;  // may be >= ntiles: dummy tile (no valid board)
             const uint32_t pos0 = tile * 2;
-            const bool valid = pos0 + brd < p.n;
-            // ---- layer-0 operand: im2col of the two bit planes, K index = tap*2 + plane, padded to 32 ----
-            build_layer0_operand(sm + kOffA0, valid ? p.own[pos0 + brd] : 0, valid ? p.enemy[pos0 + brd] : 0, 2 * h, g, x, y);
-            fence_proxy_async();
-            mbar_arrive(bar_a);
-
-            float hp0 = 0.f, hp1 = 0.f, hvv = 0.f;
+            {   // ---- layer-0 operand: im2col of the two bit planes, K index = tap*2 + plane, padded to 32 ----
+                const int m = et & 127, g = m >> 3, brd = g & 1;
+                const bool valid = pos0 + brd < p.n;
+                build_layer0_operand(sm + kOffA0, valid ? p.own[pos0 + brd] : 0, valid ? p.enemy[pos0 + brd] : 0, 2 * (et >> 7), g, m & 7,
+                                     g >> 1);
+                fence_proxy_async();
+            }
+            float hs[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};   // head partial sums: (policy 0, policy 1, value) x (board 0, 1)
             for (int l = 0; l < L; ++l) {
                 // stage this layer's folded BN parameters (double-buffered across layers)
                 float* sc = ss_s + ss_buf * 512;
                 sc[et] = __ldg(p.ss + (size_t)l * 512 + et);
                 sc[256 + et] = __ldg(p.ss + (size_t)l * 512 + 256 + et);
                 ss_buf ^= 1;
-                epi_bar();
-                mbar_wait(bar_acc, acc_par);
-                acc_par ^= 1;
-                tc_fence_after();
-                if (EXP == 1) {
-                    if (l != L - 1) { tc_fence_before(); mbar_arrive(bar_a); }
-                    continue;
+                epi_bar();   // operand (written by both warpgroups, made visible to the async proxy) and BN params ready
+                acc_fence(d);
+                if (l == 0) {
+                    mbar_wait(bar_w0, 0);
+                    wgmma_fence();
+#pragma unroll
+                    for (uint32_t j = 0; j < 2; ++j)
+                        wgmma_m64n256k16(d, smem_desc(base + kOffA0 + j * 2 * 2048 + wg * 1024, 2048, 128),
+                                         smem_desc(base + kOffW0 + j * 2 * 4096, 4096, 128), j);
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                } else {
+                    int prev = -1;
+                    for (uint32_t tap = 0; tap < 9; ++tap) {
+                        // tap (kh, kw) reads input pixel (y + kh - 1, x + kw - 1): slot offset 2*kh, chunk offset kw
+                        const uint32_t a_tap = a_wg + (2 * (tap / 3)) * kActSlot + (tap % 3) * 16;
+                        for (uint32_t kb = 0; kb < 4; ++kb) {
+                            mbar_wait(bar_full(stage), phase);
+                            const uint32_t b_st = base + kOffW + stage * kStageBytes;
+                            wgmma_fence();
+#pragma unroll
+                            for (uint32_t j = 0; j < 4; ++j)
+                                wgmma_m64n256k16(d, smem_desc(a_tap + (kb * 8 + 2 * j) * kActCg, kActCg, kActSlot),
+                                                 smem_desc(b_st + 2 * j * 4096, 4096, 128), (tap | kb | j) != 0);
+                            wgmma_commit();
+                            wgmma_wait<1>();   // the previous stage's MMAs have completed: its slot may be refilled
+                            if (prev >= 0 && lane == 0) {
+                                mbar_arrive(bar_empty(prev));
+                                if (CL > 1) mbar_arrive_cta(bar_empty(prev), crank ^ 1u);
+                            }
+                            prev = (int)stage;
+                            if (++stage == kStages) { stage = 0; phase ^= 1; }
+                        }
+                    }
+                    wgmma_wait<0>();
+                    if (lane == 0) {
+                        mbar_arrive(bar_empty(prev));
+                        if (CL > 1) mbar_arrive_cta(bar_empty(prev), crank ^ 1u);
+                    }
                 }
+                acc_fence(d);
                 const bool is_conv2 = l > 0 && (l & 1) == 0;   // second conv of a block: add the skip connection
-                const bool keep_res = l == 0 || is_conv2;      // block output: keep fp32 copy in TMEM
+                const bool keep_res = l == 0 || is_conv2;      // block output: keep an fp32 copy for the skip connection
                 const bool last = l == L - 1;
-                // 4 chunks of 32 accumulator columns per thread; the TMEM load of chunk c+1 is in flight while chunk c
-                // is processed (tcgen05.wait::ld only after the math and the stores of chunk c).
-                uint32_t va[32], vb[32], rr[32];
-                auto prefetch = [&](int c4, uint32_t (&v)[32], uint32_t (&r)[32]) {
-                    const int c0 = h * 128 + c4 * 32;
-                    tmem_ld32(tm_acc + lane_sel + c0, v);
-                    if (is_conv2) tmem_ld32(tm_res + lane_sel + c0, r);
-                };
-                auto math = [&](int c4, uint32_t (&v)[32], uint32_t (&r)[32]) {
-                    epi_math(v, r, sc, h * 128 + c4 * 32, is_conv2, keep_res || last);
-                };
-                auto store = [&](int c4, uint32_t (&v)[32]) {
-                    const int c0 = h * 128 + c4 * 32;
-                    if (keep_res && !last) tmem_st32(tm_res + lane_sel + c0, v);
-                    if (!last) epi_store_operand(v, act_row, c0 >> 3, keep_res);
-                    else epi_head_partial(v, c0, p, hp0, hp1, hvv,
-                                          (p.dbg_tower && valid) ? p.dbg_tower + ((size_t)(pos0 + brd) * 64 + y * 8 + x) * 256 : nullptr);
-                };
-                // the residual buffer rr is consumed by math(c) before prefetch(c+1) refills it
-                prefetch(0, va, rr);
-                tmem_wait_ld_dep(va); if (is_conv2) tmem_dep(rr);
-                math(0, va, rr); prefetch(1, vb, rr); store(0, va);
-                tmem_wait_ld_dep(vb); if (is_conv2) tmem_dep(rr);
-                math(1, vb, rr); prefetch(2, va, rr); store(1, vb);
-                tmem_wait_ld_dep(va); if (is_conv2) tmem_dep(rr);
-                math(2, va, rr); prefetch(3, vb, rr); store(2, va);
-                tmem_wait_ld_dep(vb); if (is_conv2) tmem_dep(rr);
-                math(3, vb, rr); store(3, vb);
-                if (!last) {
-                    if (keep_res) tmem_wait_st();
-                    fence_proxy_async();
-                    tc_fence_before();
-                    mbar_arrive(bar_a);
+                if (!last) epi_bar();   // both warpgroups' MMAs have finished reading the operand it is about to overwrite
+                float* dbg0 = nullptr;
+                float* dbg1 = nullptr;
+                if (last && p.dbg_tower) {
+                    if (pos0 < p.n) dbg0 = p.dbg_tower + ((size_t)pos0 * 64 + y * 8 + x) * 256;
+                    if (pos0 + 1 < p.n) dbg1 = p.dbg_tower + ((size_t)(pos0 + 1) * 64 + y * 8 + x) * 256;
                 }
+#pragma unroll
+                for (int i = 0; i < 32; ++i) {
+                    const int c = 8 * i + cq;
+                    const float2 s = *reinterpret_cast<const float2*>(sc + c);
+                    const float2 b = *reinterpret_cast<const float2*>(sc + 256 + c);
+                    float v0 = fmaf(d[4 * i + 0], s.x, b.x), v1 = fmaf(d[4 * i + 1], s.y, b.y);
+                    float v2 = fmaf(d[4 * i + 2], s.x, b.x), v3 = fmaf(d[4 * i + 3], s.y, b.y);
+                    if (is_conv2) {
+                        const float4 r = res[i * 256];
+                        v0 += r.x; v1 += r.y; v2 += r.z; v3 += r.w;
+                    }
+                    if (keep_res || last) {
+                        v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); v2 = fmaxf(v2, 0.f); v3 = fmaxf(v3, 0.f);
+                    }
+                    if (!last) {
+                        if (keep_res) res[i * 256] = make_float4(v0, v1, v2, v3);
+                        // the first convolution of a block folds its ReLU into the fp16 convert
+                        const uint32_t h0 = keep_res ? pack_h2<false>(v0, v1) : pack_h2<true>(v0, v1);
+                        const uint32_t h1 = keep_res ? pack_h2<false>(v2, v3) : pack_h2<true>(v2, v3);
+                        const uint32_t off = (c >> 3) * kActCg;
+                        asm volatile("st.shared.b32 [%0], %1;" ::"r"(act_row0 + off), "r"(h0) : "memory");
+                        asm volatile("st.shared.b32 [%0], %1;" ::"r"(act_row1 + off), "r"(h1) : "memory");
+                    } else {  // tower output feeds the 1x1 head convolutions (policy: 2 filters, value: 1)
+                        const float2 wa = __ldg(reinterpret_cast<const float2*>(wpc) + c);
+                        const float2 wb = __ldg(reinterpret_cast<const float2*>(wpc) + c + 1);
+                        const float va = __ldg(wvc + c), vb = __ldg(wvc + c + 1);
+                        hs[0] = fmaf(v1, wb.x, fmaf(v0, wa.x, hs[0]));
+                        hs[1] = fmaf(v1, wb.y, fmaf(v0, wa.y, hs[1]));
+                        hs[2] = fmaf(v1, vb, fmaf(v0, va, hs[2]));
+                        hs[3] = fmaf(v3, wb.x, fmaf(v2, wa.x, hs[3]));
+                        hs[4] = fmaf(v3, wb.y, fmaf(v2, wa.y, hs[4]));
+                        hs[5] = fmaf(v3, vb, fmaf(v2, va, hs[5]));
+                        if (dbg0) *reinterpret_cast<float2*>(dbg0 + c) = make_float2(v0, v1);
+                        if (dbg1) *reinterpret_cast<float2*>(dbg1 + c) = make_float2(v2, v3);
+                    }
+                }
+                if (!last) fence_proxy_async();
             }
-            // ---- heads (agent/model.py:43-56) on the 256 epilogue threads --------------------------------
-            heads_phase(p, hp0, hp1, hvv, h, m, brd, y, x, et, warp - 2, lane, pos0, part, hp, hv, logit, fc1);
-            // the next tile's layer-0 operand build only touches the A0 region, whose last reader (this tile's
-            // layer-0 MMAs) completed before the first bar_acc of this tile
+            // ---- heads (agent/model.py:43-56) on the 256 math threads ----------------------------------
+            // the four lanes of a row quad hold disjoint column sets of the same two rows
+#pragma unroll
+            for (int k = 0; k < 6; ++k) {
+                hs[k] += __shfl_xor_sync(0xffffffffu, hs[k], 1);
+                hs[k] += __shfl_xor_sync(0xffffffffu, hs[k], 2);
+            }
+            // lane quad (0, 1, 2, 3) -> (row r0 colhalf 0, row r0 + 8 colhalf 0, r0 colhalf 1 = 0, r0 + 8 colhalf 1 = 0)
+            const int q = lane & 3, brd = q & 1, m = r0 + 8 * brd;
+            const bool full = q < 2;
+            heads_phase(p, full ? hs[3 * brd] : 0.f, full ? hs[3 * brd + 1] : 0.f, full ? hs[3 * brd + 2] : 0.f, q >> 1, m, brd, y, x, et,
+                        warp, lane, pos0, part, hp, hv, logit, fc1);
         }
     }
 
-    tc_fence_before();
     __syncthreads();
     if (CL > 1) cluster_sync_all();  // no CTA leaves while a peer may still multicast into it / arrive on its barriers
-    if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem) : "memory");
 }
 
 // ---- weight packing -----------------------------------------------------------------------------------
@@ -292,22 +300,38 @@ int net_pack_tc(rz_net* net, cudaStream_t stream) {
     return RZ_OK;
 }
 
+static std::mutex g_res_mutex;   // orders the tower launches that share a network's residual scratch
+static int g_cluster = 0;        // 0: not yet decided (RZ_TOWER_CLUSTER, default 2)
+
+int set_tower_cluster(int cluster) {
+    RZ_REQUIRE(cluster == 1 || cluster == 2, "rz_net_set_tower_cluster: cluster must be 1 or 2");
+    g_cluster = cluster;
+    return RZ_OK;
+}
+
 int net_forward_tc(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value, size_t n, cudaStream_t stream,
                    float* dbg_tower, const uint32_t* n_dev, float* dbg_logits, float* dbg_vlogit) {
-    RZ_REQUIRE(net->cfg.filters == 256, "tcgen05 tower requires 256 filters");
-    RZ_REQUIRE(net->cfg.value_fc <= (int)tc::kMaxV, "tcgen05 tower supports value_fc_size <= %u", tc::kMaxV);
+    RZ_REQUIRE(net->cfg.filters == 256, "wgmma tower requires 256 filters");
+    RZ_REQUIRE(net->cfg.value_fc <= (int)tc::kTcMaxV, "wgmma tower supports value_fc_size <= %u", tc::kTcMaxV);
     RZ_REQUIRE(n < (1ull << 31), "batch too large");
-    static int cluster = -1, experiment = 0;
-    if (cluster < 0) {
-        const char* cs = getenv("RZ_TOWER_CLUSTER");
-        cluster = (cs && atoi(cs) == 1) ? 1 : 2;
-        const char* ex = getenv("RZ_TOWER_EXPERIMENT");
-        experiment = ex ? atoi(ex) : 0;
-        RZ_CUDA_TRY(cudaFuncSetAttribute(tc::net_tower_kernel<2, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc::kSmemAlloc));
-        RZ_CUDA_TRY(cudaFuncSetAttribute(tc::net_tower_kernel<2, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc::kSmemAlloc));
+    static int max_pairs = -1;
+    if (max_pairs < 0) {
         RZ_CUDA_TRY(cudaFuncSetAttribute(tc::net_tower_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc::kSmemAlloc));
         RZ_CUDA_TRY(cudaFuncSetAttribute(tc::net_tower_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc::kSmemAlloc));
+        // how many CTA pairs can be resident at once: an SM without a free partner in its GPC cannot take a pair
+        cudaLaunchConfig_t cfg = {};
+        cfg.gridDim = dim3((unsigned)num_sms() & ~1u); cfg.blockDim = dim3(tc::kThreads); cfg.dynamicSmemBytes = tc::kSmemAlloc;
+        cudaLaunchAttribute attr[1];
+        attr[0].id = cudaLaunchAttributeClusterDimension;
+        attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+        cfg.attrs = attr; cfg.numAttrs = 1;
+        RZ_CUDA_TRY(cudaOccupancyMaxActiveClusters(&max_pairs, tc::net_tower_kernel<2>, &cfg));
     }
+    if (g_cluster == 0) {
+        const char* cs = getenv("RZ_TOWER_CLUSTER");
+        g_cluster = (cs && atoi(cs) == 1) ? 1 : 2;
+    }
+    const int cluster = g_cluster == 2 && max_pairs >= 1 ? 2 : 1;
     tc::Params p;
     p.w0 = net->tc_w0; p.w = net->tc_w; p.ss = net->scale_shift; p.blob = net->blob;
     p.off_policy_conv = net->off_policy_conv; p.off_policy_fc_k = net->off_policy_fc_k; p.off_policy_fc_b = net->off_policy_fc_b;
@@ -316,23 +340,26 @@ int net_forward_tc(rz_net* net, const uint64_t* own, const uint64_t* enemy, floa
     p.own = own; p.enemy = enemy; p.policy = policy; p.value = value; p.dbg_tower = dbg_tower;
     p.dbg_logits = dbg_logits; p.dbg_vlogit = dbg_vlogit;
     p.n = (uint32_t)n; p.n_dev = n_dev; p.n_layers = 1 + 2 * net->cfg.res_blocks; p.V = net->cfg.value_fc;
+    p.res = net->res;
+    std::lock_guard<std::mutex> lock(g_res_mutex);
+    RZ_CUDA_TRY(cudaStreamWaitEvent(stream, net->res_done, 0));   // the previous launch on this scratch, whatever its stream
     const uint32_t ntiles = (uint32_t)((n + 1) / 2);
     uint32_t grid = ntiles < (uint32_t)num_sms() ? ntiles : (uint32_t)num_sms();
     if (cluster == 1) {
         tc::net_tower_kernel<1><<<grid, tc::kThreads, tc::kSmemAlloc, stream>>>(p);
     } else {
         grid = (grid + 1) & ~1u;  // whole clusters; a surplus CTA runs dummy tiles
+        if (grid > 2u * (uint32_t)max_pairs) grid = 2u * (uint32_t)max_pairs;
         cudaLaunchConfig_t cfg = {};
         cfg.gridDim = dim3(grid); cfg.blockDim = dim3(tc::kThreads); cfg.dynamicSmemBytes = tc::kSmemAlloc; cfg.stream = stream;
         cudaLaunchAttribute attr[1];
         attr[0].id = cudaLaunchAttributeClusterDimension;
         attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
         cfg.attrs = attr; cfg.numAttrs = 1;
-        if (experiment == 1) RZ_CUDA_TRY(cudaLaunchKernelEx(&cfg, tc::net_tower_kernel<2, 1>, p));
-        else if (experiment == 2) RZ_CUDA_TRY(cudaLaunchKernelEx(&cfg, tc::net_tower_kernel<2, 2>, p));
-        else RZ_CUDA_TRY(cudaLaunchKernelEx(&cfg, tc::net_tower_kernel<2>, p));
+        RZ_CUDA_TRY(cudaLaunchKernelEx(&cfg, tc::net_tower_kernel<2>, p));
     }
     RZ_LAUNCH_CHECK();
+    RZ_CUDA_TRY(cudaEventRecord(net->res_done, stream));
     return RZ_OK;
 }
 

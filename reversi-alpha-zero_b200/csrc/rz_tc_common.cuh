@@ -1,6 +1,5 @@
-// rz_tc_common.cuh -- PTX wrappers (mbarrier, bulk copy, tcgen05 MMA / TMEM load-store / commit, cluster) and the
-// parameter block shared by the two tcgen05 tower kernels (rz_net_tc.cu: one CTA per tile, cta_group::1;
-// rz_net_tc2.cu: CTA pairs, cta_group::2, epilogue overlapped with the MMA stream).
+// rz_tc_common.cuh -- PTX wrappers (mbarrier, bulk copy with cluster multicast, wgmma) and the pieces of the fused
+// tower kernel (rz_net_tc.cu) that do not depend on its pipeline: parameter block, layer-0 operand, heads.
 #pragma once
 #include <cuda_fp16.h>
 #include "rz_bitboard.cuh"
@@ -15,11 +14,17 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)_
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
 }
+__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+// arrive on the barrier at the same offset in CTA `rank` of the cluster
+__device__ __forceinline__ void mbar_arrive_cta(uint32_t bar, uint32_t rank) {
+    uint32_t remote;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(bar), "r"(rank));
+    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
 }
 // Bounded wait (~4 s of SM clocks): a protocol bug traps and is reported to the host instead of hanging the GPU.
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
@@ -45,17 +50,13 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
                  "r"(bytes), "r"(bar)
                  : "memory");
 }
-// multicast variants (thread-block cluster): the copy lands at the same CTA-relative offset in every CTA of
-// `mask` and signals the mbarrier at the same offset there; the commit arrives on every CTA's barrier
+// multicast variant (thread-block cluster): the copy lands at the same CTA-relative offset in every CTA of `mask` and
+// signals the mbarrier at the same offset there
 __device__ __forceinline__ void bulk_g2s_mc(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar, uint16_t mask) {
     asm volatile(
         "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;" ::"r"(dst),
         "l"(src), "r"(bytes), "r"(bar), "h"(mask)
         : "memory");
-}
-__device__ __forceinline__ void umma_commit_mc(uint32_t bar, uint16_t mask) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar), "h"(mask)
-                 : "memory");
 }
 __device__ __forceinline__ void cluster_sync_all() {
     asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
@@ -66,73 +67,48 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
     return r;
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// named barrier of the 256 math threads (warps 0..7)
 __device__ __forceinline__ void epi_bar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
-// shared-memory matrix descriptor: K-major, SWIZZLE_NONE; core matrix = 8 rows x 16 B (rows 16 B apart);
-// LBO = byte distance between the two K-halves of one MMA, SBO = byte distance between 8-row groups.
+// wgmma shared-memory matrix descriptor: K-major, no swizzle; core matrix = 8 rows x 16 B (rows 16 B apart);
+// LBO = byte distance between core matrices adjacent in K, SBO = byte distance between 8-row groups.
 __device__ __forceinline__ uint64_t smem_desc(uint32_t addr, uint32_t lbo, uint32_t sbo) {
-    return (uint64_t)((addr >> 4) & 0x3FFF) | ((uint64_t)((lbo >> 4) & 0x3FFF) << 16) | ((uint64_t)((sbo >> 4) & 0x3FFF) << 32) |
-           (1ULL << 46);
+    return (uint64_t)((addr >> 4) & 0x3FFF) | ((uint64_t)((lbo >> 4) & 0x3FFF) << 16) | ((uint64_t)((sbo >> 4) & 0x3FFF) << 32);
 }
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// pins the accumulator registers at this point of the instruction stream (no use or definition moves across)
+__device__ __forceinline__ void acc_fence(float (&d)[128]) {
+#pragma unroll
+    for (int i = 0; i < 128; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
+#define RZ_D4(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3])
+#define RZ_D16(i) RZ_D4(i), RZ_D4(i + 4), RZ_D4(i + 8), RZ_D4(i + 12)
+// D[64 x 256] (+)= A[64 x 16] * B[16 x 256]: fp16 operands from shared memory (both K-major), fp32 accumulators in
+// registers; accumulate = 0 overwrites D.
+__device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-          "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]),
-          "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-          "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr)
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %130, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+        "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+        "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+        "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+        "}, %128, %129, p, 1, 1, 0, 0;\n\t}"
+        : RZ_D16(0), RZ_D16(16), RZ_D16(32), RZ_D16(48), RZ_D16(64), RZ_D16(80), RZ_D16(96), RZ_D16(112)
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
         : "memory");
 }
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-        "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]), "r"(v[10]),
-        "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]), "r"(v[19]), "r"(v[20]),
-        "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]), "r"(v[28]), "r"(v[29]), "r"(v[30]),
-        "r"(v[31])
-        : "memory");
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// wait::ld that also carries a register dependency on the loaded values, so the compiler cannot schedule a use of
-// v[] above the wait (tcgen05.ld completes asynchronously)
-__device__ __forceinline__ void tmem_wait_ld_dep(uint32_t (&v)[32]) {
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-                 : "+r"(v[0]), "+r"(v[1]), "+r"(v[2]), "+r"(v[3]), "+r"(v[4]), "+r"(v[5]), "+r"(v[6]), "+r"(v[7]), "+r"(v[8]), "+r"(v[9]),
-                   "+r"(v[10]), "+r"(v[11]), "+r"(v[12]), "+r"(v[13]), "+r"(v[14]), "+r"(v[15]), "+r"(v[16]), "+r"(v[17]), "+r"(v[18]),
-                   "+r"(v[19]), "+r"(v[20]), "+r"(v[21]), "+r"(v[22]), "+r"(v[23]), "+r"(v[24]), "+r"(v[25]), "+r"(v[26]), "+r"(v[27]),
-                   "+r"(v[28]), "+r"(v[29]), "+r"(v[30]), "+r"(v[31])
-                 :
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_dep(uint32_t (&v)[32]) {
-    asm volatile(""
-                 : "+r"(v[0]), "+r"(v[1]), "+r"(v[2]), "+r"(v[3]), "+r"(v[4]), "+r"(v[5]), "+r"(v[6]), "+r"(v[7]), "+r"(v[8]), "+r"(v[9]),
-                   "+r"(v[10]), "+r"(v[11]), "+r"(v[12]), "+r"(v[13]), "+r"(v[14]), "+r"(v[15]), "+r"(v[16]), "+r"(v[17]), "+r"(v[18]),
-                   "+r"(v[19]), "+r"(v[20]), "+r"(v[21]), "+r"(v[22]), "+r"(v[23]), "+r"(v[24]), "+r"(v[25]), "+r"(v[26]), "+r"(v[27]),
-                   "+r"(v[28]), "+r"(v[29]), "+r"(v[30]), "+r"(v[31])
-                 :
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
+#undef RZ_D16
+#undef RZ_D4
 
 // two fp32 -> packed fp16x2 (a in the low half), saturating at +-65504; RELU folds max(x, 0) into the convert
 template <bool RELU>
@@ -154,6 +130,7 @@ struct Params {
     const u64* enemy;
     float* policy;
     float* value;
+    float* res;        // fp32 residual stream, [CTA][32][256 threads][4]
     float* dbg_tower;  // nullable
     float* dbg_logits; // nullable: [n][64] policy logits (before the softmax)
     float* dbg_vlogit; // nullable: [n] value before the tanh
@@ -163,8 +140,6 @@ struct Params {
     int V;
 };
 
-// ---- pieces of the epilogue shared by the two tower kernels (rz_net_tc.cu, rz_net_tc2.cu) ----------------------------
-constexpr uint32_t kTcActCg = 2896;   // byte distance between channel groups of 8 in the operand layout
 constexpr uint32_t kTcMaxV = 512;
 
 // layer-0 operand (agent/model.py:30-33 first convolution as a GEMM): im2col of the two bit planes of one board row m =
@@ -194,67 +169,10 @@ __device__ __forceinline__ void build_layer0_operand(uint8_t* a0, u64 o, u64 e, 
     }
 }
 
-// folded BatchNorm (+ skip connection + ReLU) on 32 accumulator columns c0 .. c0 + 31 of one row; sc = [scale 256][shift 256].
-// conv2: second convolution of a block (adds the fp32 residual r, ReLU); relu_now: block outputs / the last layer (ReLU here);
-// otherwise the first convolution of a block, whose ReLU is folded into the fp16 convert of epi_store_operand
-__device__ __forceinline__ void epi_math(uint32_t (&v)[32], const uint32_t (&r)[32], const float* sc, int c0, bool conv2, bool relu_now) {
-    if (conv2) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j)
-            v[j] = __float_as_uint(fmaxf(fmaf(__uint_as_float(v[j]), sc[c0 + j], sc[256 + c0 + j]) + __uint_as_float(r[j]), 0.f));
-    } else if (relu_now) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(fmaxf(fmaf(__uint_as_float(v[j]), sc[c0 + j], sc[256 + c0 + j]), 0.f));
-    } else {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(fmaf(__uint_as_float(v[j]), sc[c0 + j], sc[256 + c0 + j]));
-    }
-}
-
-// 32 fp32 values of one row -> fp16, four 16-byte chunks (8 channels each) at row_addr + (cg0 + jj) * kTcActCg
-__device__ __forceinline__ void epi_store_operand(const uint32_t (&v)[32], uint32_t row_addr, int cg0, bool already_relu) {
-#pragma unroll
-    for (int jj = 0; jj < 4; ++jj) {
-        uint4 pk;
-        if (already_relu) {
-            pk.x = pack_h2<false>(__uint_as_float(v[jj * 8 + 0]), __uint_as_float(v[jj * 8 + 1]));
-            pk.y = pack_h2<false>(__uint_as_float(v[jj * 8 + 2]), __uint_as_float(v[jj * 8 + 3]));
-            pk.z = pack_h2<false>(__uint_as_float(v[jj * 8 + 4]), __uint_as_float(v[jj * 8 + 5]));
-            pk.w = pack_h2<false>(__uint_as_float(v[jj * 8 + 6]), __uint_as_float(v[jj * 8 + 7]));
-        } else {
-            pk.x = pack_h2<true>(__uint_as_float(v[jj * 8 + 0]), __uint_as_float(v[jj * 8 + 1]));
-            pk.y = pack_h2<true>(__uint_as_float(v[jj * 8 + 2]), __uint_as_float(v[jj * 8 + 3]));
-            pk.z = pack_h2<true>(__uint_as_float(v[jj * 8 + 4]), __uint_as_float(v[jj * 8 + 5]));
-            pk.w = pack_h2<true>(__uint_as_float(v[jj * 8 + 6]), __uint_as_float(v[jj * 8 + 7]));
-        }
-        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(row_addr + (cg0 + jj) * kTcActCg), "r"(pk.x), "r"(pk.y), "r"(pk.z),
-                     "r"(pk.w)
-                     : "memory");
-    }
-}
-
-// tower output columns c0 .. c0 + 31 of one row feed the 1x1 head convolutions from registers (policy: 2 filters, value: 1)
-__device__ __forceinline__ void epi_head_partial(const uint32_t (&v)[32], int c0, const Params& p, float& hp0, float& hp1, float& hvv,
-                                                 float* dbg_row /* nullable: this row's 256 tower outputs */) {
-    const float* wp = p.blob + p.off_policy_conv;
-    const float* wv = p.blob + p.off_value_conv;
-#pragma unroll
-    for (int j = 0; j < 32; ++j) {
-        const float a = __uint_as_float(v[j]);
-        const float2 w2 = __ldg(reinterpret_cast<const float2*>(wp) + c0 + j);
-        hp0 = fmaf(a, w2.x, hp0);
-        hp1 = fmaf(a, w2.y, hp1);
-        hvv = fmaf(a, __ldg(wv + c0 + j), hvv);
-    }
-    if (dbg_row) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) dbg_row[c0 + j] = __uint_as_float(v[j]);
-    }
-}
-
-// heads (agent/model.py:43-56) on the 256 epilogue threads of a CTA for its two boards: the per-thread partial sums of the
-// two column halves (colhalf 0 / 1 of row m) -> BN + ReLU -> Dense(128 -> 64) + softmax, Dense(64 -> V) + ReLU -> Dense(V -> 1)
-// + tanh.  part [2][128][4], hp [2][128], hv [2][64], logit [2][64], fc1 [2][kTcMaxV]: shared-memory scratch.
+// heads (agent/model.py:43-56) on the 256 math threads of a CTA for its two boards: per-row partial sums of the 1x1 head
+// convolutions over two column halves (colhalf 0 / 1 of row m) -> BN + ReLU -> Dense(128 -> 64) + softmax,
+// Dense(64 -> V) + ReLU -> Dense(V -> 1) + tanh.  part [2][128][4], hp [2][128], hv [2][64], logit [2][64],
+// fc1 [2][kTcMaxV]: shared-memory scratch.
 __device__ __forceinline__ void heads_phase(const Params& p, float hp0, float hp1, float hvv, int colhalf, int m, int brd, int y, int x,
                                             int et, int ew, int lane, uint32_t pos0, float* part, float* hp, float* hv, float* logit,
                                             float* fc1) {

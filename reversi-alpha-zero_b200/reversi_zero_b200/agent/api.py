@@ -1,6 +1,6 @@
 """Mirror of the reference's ``ReversiModelAPI`` (agent/api.py:20-45): ``predict(x)`` with
 ``x`` = ``(2,8,8)`` or ``(N,2,8,8)`` planes ``[own, enemy]`` of the side to move, returning
-``(policy (64,)|(N,64), value (1,)|(N,1))`` -- evaluated by the CUDA network (tcgen05 tower for the
+``(policy (64,)|(N,64), value (1,)|(N,1))`` -- evaluated by the CUDA network (wgmma tower for the
 256-filter model).  The multi-process pipe server of the reference (agent/api.py:48-141) has no
 equivalent: batching happens on the device inside the engine."""
 import numpy as np

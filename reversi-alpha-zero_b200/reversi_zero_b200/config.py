@@ -1,5 +1,5 @@
 """Configuration tree with the reference's field names and defaults (config.py:15-193) so that the
-reference's YAML files (config/*.yml) and its own ``Config`` objects drive the B200 engine unchanged.
+reference's YAML files (config/*.yml) and its own ``Config`` objects drive the H100 engine unchanged.
 Only the sections the self-play path reads are modelled; any object exposing the same attributes
 (e.g. the reference's ``Config`` built by moke_config) is accepted everywhere in this package.
 

@@ -1,6 +1,6 @@
 """Mirror of the reference's ``reversi_zero.lib.bitboard`` free functions (lib/bitboard.py) over the
 C ABI.  Scalar calls use the host twins of the device code (csrc/rz_bitboard.cuh compiled for the
-host); the ``*_batch`` functions run the sm_100a K1 kernels on numpy arrays (host buffers) and are
+host); the ``*_batch`` functions run the sm_90a K1 kernels on numpy arrays (host buffers) and are
 what the parity tests and the microbenchmark exercise."""
 import ctypes as C
 

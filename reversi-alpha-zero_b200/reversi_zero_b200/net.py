@@ -9,9 +9,10 @@ from .agent import model as M
 IMPL_AUTO, IMPL_GENERIC, IMPL_TCGEN05 = 0, 1, 2
 
 
-def set_tower_kernel(version):
-    """1 = one CTA per tile, 2 = CTA pairs with overlapped epilogue (rz_net_set_tower_kernel); process-wide"""
-    _cabi.check(_cabi.lib().rz_net_set_tower_kernel(int(version)), "rz_net_set_tower_kernel")
+def set_tower_cluster(cluster):
+    """2 = the tower kernel in CTA pairs sharing the weight stages (default), 1 = single CTAs (rz_net_set_tower_cluster);
+    process-wide"""
+    _cabi.check(_cabi.lib().rz_net_set_tower_cluster(int(cluster)), "rz_net_set_tower_cluster")
 
 
 class Net:
@@ -66,7 +67,7 @@ class Net:
                                                         C.c_void_p(tower_t.data_ptr()), n, stream_ptr), "rz_net_debug_tower_dev")
 
     def debug_heads_dev(self, own_t, enemy_t, policy_t, value_t, logits_t, vlogit_t, n, tower_t=None, stream_ptr=None):
-        """tcgen05 path with the head outputs before softmax / tanh (and optionally the fp32 tower output)"""
+        """tensor-core tower path with the head outputs before softmax / tanh (and optionally the fp32 tower output)"""
         _cabi.check(_cabi.lib().rz_net_debug_heads_dev(self._h, C.c_void_p(own_t.data_ptr()), C.c_void_p(enemy_t.data_ptr()),
                                                         C.c_void_p(policy_t.data_ptr()), C.c_void_p(value_t.data_ptr()),
                                                         C.c_void_p(tower_t.data_ptr()) if tower_t is not None else None,

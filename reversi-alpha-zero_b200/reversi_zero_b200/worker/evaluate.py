@@ -1,4 +1,4 @@
-"""Mirror of the reference's evaluator (worker/evaluate.py:17-124) on the B200 engine: the challenger
+"""Mirror of the reference's evaluator (worker/evaluate.py:17-124) on the H100 engine: the challenger
 ("next generation") network plays ``eval.game_num`` games against the best network and replaces it when its
 winning rate over the decided games reaches ``eval.replace_rate``.
 

@@ -1,4 +1,4 @@
-"""Mirror of the reference's self-play worker (worker/self_play.py) on the B200 engine.
+"""Mirror of the reference's self-play worker (worker/self_play.py) on the H100 engine.
 
 ``start(config)`` / ``SelfPlayWorker(config, env, api, shared_var, worker_index).start()`` keep the
 reference's entry points (manager.py:51-53, worker/self_play.py:28-41,64-93) and output contract:

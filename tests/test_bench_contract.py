@@ -1,5 +1,5 @@
 """bench.py's reference arm (CPU side of the contract): `--impl reference --steps K --warmup W` honours K and W, prints
-one JSON line on the real stdout and describes the SAME workload (`config`) as the B200 arm.  No GPU involved."""
+one JSON line on the real stdout and describes the SAME workload (`config`) as the CUDA arm.  No GPU involved."""
 import argparse
 import json
 import os
@@ -45,7 +45,7 @@ def test_reference_arm_line_and_shared_config():
 
 
 def test_reference_arm_under_torchrun_prints_one_line_from_rank_0():
-    """the driver launches the reference arm like the B200 arm (torchrun, one rank per GPU): rank 0 alone measures and prints,
+    """the driver launches the reference arm like the CUDA arm (torchrun, one rank per GPU): rank 0 alone measures and prints,
     the other ranks exit 0 without work"""
     env = dict(os.environ, RZ_BENCH_REFERENCE_TOTAL_S="6", CUDA_VISIBLE_DEVICES="")
     r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr", "127.0.0.1",

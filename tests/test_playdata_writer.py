@@ -70,28 +70,35 @@ def test_float_repr_edge_cases(tmp_path):
             assert repr(float(v)) in text
 
 
-def test_reference_trainer_loads_our_files(tmp_path):
-    """SURVEY 8(c)(v): a play_data file written by the C-ABI writer goes through the UNMODIFIED reference's
-    read_game_data_from_file + OptimizeWorker.convert_to_training_data (worker/optimize.py:215-231).  Runs only where
-    the reference checkout exists (the build container)."""
-    import oracle.ref_shims.install as shims
-    if not shims.available():
-        pytest.skip("reference sources not present")
-    shims.install()
-    from reversi_zero.lib.data_helper import read_game_data_from_file
-    from reversi_zero.worker.optimize import OptimizeWorker
+def fixed_games():
+    """two seeded games of the oracle's self-play (fake network): the input of the trainer comparison"""
     pp = mcts.PlayParams(simulation_num_per_move=20, parallel_search_num=4, noise_eps=0.25, c_puct=5)
-    games = [mcts.SelfPlayGame(pp, onn.FakeNetAPI(), seed=5, game_id=i).play() for i in range(2)]
+    return [mcts.SelfPlayGame(pp, onn.FakeNetAPI(), seed=5, game_id=i).play() for i in range(2)]
+
+
+def test_reference_trainer_loads_our_files(tmp_path, golden_dir):
+    """SURVEY 8(c)(v): a play_data file written by the C-ABI writer, as the UNMODIFIED reference's
+    read_game_data_from_file + OptimizeWorker.convert_to_training_data (worker/optimize.py:215-231) loads it -- its output on
+    this fixed two-game file is stored in tests/golden/trainer_ref.npz (tests/golden/make_golden_host_ref.py) -- equals what the
+    trainer-side loader restatement (oracle/ingest.py, the JSON records of the same file) gives."""
+    games = fixed_games()
     G, P = to_ctypes(games)
     path = str(tmp_path / "play_20260922-000000.000000.json")
     n = E.write_play_data(path, G, len(games), P, True, 4)
-    data = read_game_data_from_file(path)
-    states, policies, zs = OptimizeWorker.convert_to_training_data(data)
+    ref = np.load(f"{golden_dir}/trainer_ref.npz")
+    states, policies, zs = ref["states"], ref["policies"], ref["zs"]
     assert states.shape == (n, 2, 8, 8) and policies.shape == (n, 64) and zs.shape == (n,)
     assert states.dtype == np.uint8 and set(np.unique(zs)) <= {-1, 0, 1}
     assert np.allclose(policies.sum(axis=1), 1.0)
     # first record = first ply of black from the start position, identity symmetry
     assert states[0, 0].sum() == 2 and states[0, 1].sum() == 2 and states[0, 0, 3, 4] == 1
+    # the same arrays from our file, read the way the trainer reads it (agent/player.py records -> convert_to_training_data)
+    data = json.loads(open(path).read())
+    mine_states = np.array([[ob.bit_to_array(o, 64).reshape(8, 8), ob.bit_to_array(e, 64).reshape(8, 8)] for (o, e), _, _ in data],
+                           dtype=np.uint8)
+    assert np.array_equal(mine_states, states)
+    assert np.array_equal(np.array([p for _, p, _ in data]), policies)
+    assert np.array_equal(np.array([z for _, _, z in data]), zs)
 
 
 def test_ply_without_visits_does_not_crash(tmp_path):

@@ -1,18 +1,23 @@
-"""The reference's OWN compiled code (lib/alt/bitboard_cython.pyx, lib/alt/reversi_solver_cython.pyx, built by
-oracle/build_ref.py into oracle/_ref -- it travels to the GPU box) against
-  * the oracle restatements (CPU, here), and
+"""The reference's OWN compiled code (lib/alt/bitboard_cython.pyx, lib/alt/reversi_solver_cython.pyx) against
+  * the oracle restatements (CPU), and
   * the CUDA operators through the C ABI (GPU): K1 move generation / flips on 1 M seeded positions of the
     SURVEY 8(d) config-5 recipe, and the batched endgame solver.
-Skipped where oracle/_ref has not been built (it needs the reference checkout once)."""
+The reference's outputs on these seeded inputs are stored under tests/golden (ref_native.npz: a fixed sample of the 1 M
+positions; ref_native_solver.json: every endgame), written by tests/golden/make_golden_ref_native.py from the compiled
+reference modules."""
+import json
+import os
+
 import numpy as np
 import pytest
 
-from oracle import bitboard as ob, ref_native
+from oracle import bitboard as ob
 from oracle.solver import Solver
 
-pytestmark = pytest.mark.skipif(not ref_native.available(), reason="oracle/_ref not built")
-
 U64 = np.uint64
+N_POSITIONS = 1_000_000
+GOLDEN_SAMPLE = 32_768
+ENDGAME_SETS = dict(oracle=(120, 41), device=(200, 43))
 
 
 def config5_positions(n, seed=20260922):
@@ -29,11 +34,9 @@ def config5_positions(n, seed=20260922):
     return occ & r, occ & ~r, pos
 
 
-def reference_outputs(own, enemy, pos):
-    bb, _ = ref_native.load()
-    legal = np.fromiter((bb.find_correct_moves(int(o), int(e)) for o, e in zip(own, enemy)), dtype=U64, count=len(own))
-    flip = np.fromiter((bb.calc_flip(int(p), int(o), int(e)) for p, o, e in zip(pos, own, enemy)), dtype=U64, count=len(own))
-    return legal, flip
+def golden_sample_indices():
+    """the positions of the 1 M set whose reference outputs are stored: a fixed seeded sample across all three thirds"""
+    return np.sort(np.random.default_rng(7).choice(N_POSITIONS, GOLDEN_SAMPLE, replace=False))
 
 
 def random_endgames(n, seed, max_empties=10):
@@ -52,43 +55,54 @@ def random_endgames(n, seed, max_empties=10):
     return out
 
 
-def reference_solve(own, enemy, exactly):
-    """ReversiSolver.solve(black, white, next_player, exactly) of the compiled reference, position given in the mover's frame"""
-    _, sv = ref_native.load()
-    mv, sc = sv.ReversiSolver().solve(own, enemy, ref_native.player_enum().black, exactly=exactly)
-    return (-1, 0) if mv is None else (int(mv), int(sc))
+def reference_outputs(golden_dir):
+    """(indices, legal, flip) of the compiled reference on the stored sample of the 1 M positions"""
+    z = np.load(os.path.join(golden_dir, "ref_native.npz"))
+    return golden_sample_indices(), z["legal"], z["flip"]
 
 
-def test_oracle_bitboard_matches_compiled_reference():
-    own, enemy, pos = config5_positions(100_000)
-    legal, flip = reference_outputs(own, enemy, pos)
-    assert np.array_equal(ob.find_correct_moves_batch(own, enemy), legal)
-    assert np.array_equal(ob.calc_flip_batch(pos, own, enemy), flip)
+def reference_solves(golden_dir, name):
+    """{exactly: [(move, score)] } of ReversiSolver.solve(black, white, next_player, exactly) of the compiled reference,
+    positions given in the mover's frame, move -1 / score 0 where it returns no move"""
+    with open(os.path.join(golden_dir, "ref_native_solver.json")) as f:
+        d = json.load(f)[name]
+    return {ex: [tuple(x) for x in d[str(ex)]] for ex in (True, False)}
 
 
-def test_oracle_solver_matches_compiled_reference():
-    for own, enemy in random_endgames(120, seed=41):
+def test_oracle_bitboard_matches_compiled_reference(golden_dir):
+    own, enemy, pos = config5_positions(N_POSITIONS)
+    idx, legal, flip = reference_outputs(golden_dir)
+    assert np.array_equal(ob.find_correct_moves_batch(own[idx], enemy[idx]), legal)
+    assert np.array_equal(ob.calc_flip_batch(pos[idx], own[idx], enemy[idx]), flip)
+
+
+def test_oracle_solver_matches_compiled_reference(golden_dir):
+    ref = reference_solves(golden_dir, "oracle")
+    for i, (own, enemy) in enumerate(random_endgames(*ENDGAME_SETS["oracle"])):
         for exactly in (True, False):
             mv, sc = Solver().solve(own, enemy, exactly)
-            assert ((-1, 0) if mv is None else (mv, sc)) == reference_solve(own, enemy, exactly)
+            assert ((-1, 0) if mv is None else (mv, sc)) == ref[exactly][i]
 
 
 @pytest.mark.gpu
-def test_k1_kernels_match_compiled_reference_1m():
+def test_k1_kernels_match_compiled_reference_1m(golden_dir):
     from reversi_zero_b200.lib import bitboard as zb
-    own, enemy, pos = config5_positions(1_000_000)
-    legal, flip = reference_outputs(own, enemy, pos)
-    assert np.array_equal(zb.find_correct_moves_batch(own, enemy), legal)      # bit-exact, 1 M positions
-    assert np.array_equal(zb.calc_flip_batch(pos, own, enemy), flip)          # including occupied / illegal squares
+    own, enemy, pos = config5_positions(N_POSITIONS)
+    legal, flip = zb.find_correct_moves_batch(own, enemy), zb.calc_flip_batch(pos, own, enemy)   # 1 M positions
+    idx, ref_legal, ref_flip = reference_outputs(golden_dir)
+    assert np.array_equal(legal[idx], ref_legal)      # bit-exact against the reference on the stored sample
+    assert np.array_equal(flip[idx], ref_flip)        # including occupied / illegal squares
+    assert np.array_equal(legal, ob.find_correct_moves_batch(own, enemy))   # and against the oracle on all 1 M
+    assert np.array_equal(flip, ob.calc_flip_batch(pos, own, enemy))
 
 
 @pytest.mark.gpu
-def test_device_solver_matches_compiled_reference():
+def test_device_solver_matches_compiled_reference(golden_dir):
     from reversi_zero_b200.lib import reversi_solver as zs
-    cases = random_endgames(200, seed=43)
+    ref = reference_solves(golden_dir, "device")
+    cases = random_endgames(*ENDGAME_SETS["device"])
     own = [c[0] for c in cases]
     enemy = [c[1] for c in cases]
     for exactly in (True, False):
         mv, sc = zs.solve_batch(own, enemy, [exactly] * len(cases))
-        for o, e, m, s in zip(own, enemy, mv, sc):
-            assert (int(m), int(s)) == reference_solve(o, e, exactly)
+        assert [(int(m), int(s)) for m, s in zip(mv, sc)] == ref[exactly]

@@ -35,7 +35,7 @@ def run(n=1 << 20, iters=20, warmup=3, cpu_rows=1024):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm = peaks.get("hbm_gbs", 6650.0)
+    hbm = peaks.get("hbm_gbs", 3350.0)   # H100 SXM data-sheet HBM3 bandwidth when no measured peak is given
     rows = synth_rows(n)
     dev = torch.device("cuda", 0)
     d_rows = torch.from_numpy(rows.view(np.uint8).reshape(-1)).to(dev)

@@ -15,11 +15,6 @@ def run(n=32768, iters=5, warmup=2, res_blocks=10):
     import torch
     from reversi_zero_b200.agent import model as M
     from reversi_zero_b200 import net as N, device as D
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        pass
     mc = M.ModelConfig(res_layer_num=res_blocks)
     flop = 2 * (64 * 256 * 18 + res_blocks * 2 * 64 * 256 * 2304 + 64 * 3 * 256 + 128 * 64 + 64 * 256 + 256)
     net = N.Net(mc)
@@ -40,15 +35,15 @@ def run(n=32768, iters=5, warmup=2, res_blocks=10):
     torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / iters
     tflops = n * flop / ms / 1e9
-    return dict(n=n, res_blocks=res_blocks, flop_per_position=flop, ms=ms, pos_per_s=n / ms * 1e3, tflops=tflops, frac_of_burst_peak=tflops / peaks.get("bf16_tflops", 1590.0),
-                frac_of_sustained_peak=tflops / peaks.get("bf16_tflops_sustained", 1400.0))
+    # share of the H100 SXM data-sheet dense FP16 tensor rate (989 TFLOP/s at 700 W), not a measured peak
+    return dict(n=n, res_blocks=res_blocks, flop_per_position=flop, ms=ms, pos_per_s=n / ms * 1e3, tflops=tflops,
+                frac_of_datasheet_fp16=tflops / 989.0, gpu=torch.cuda.get_device_name())
 
 
 if __name__ == "__main__":
-    # python tools/nn_bench.py [res_blocks] [iters]; RZ_TOWER_EXPERIMENT=1|2 times the measurement variants of the kernel
+    # python tools/nn_bench.py [res_blocks] [iters]
     rb = int(sys.argv[1]) if len(sys.argv) > 1 else 10
     iters = int(sys.argv[2]) if len(sys.argv) > 2 else 5
     for n in (296, 32768):
         r = run(n, iters=iters, res_blocks=rb)
-        r["experiment"] = os.environ.get("RZ_TOWER_EXPERIMENT", "0")
         print(json.dumps(r))

@@ -6,7 +6,7 @@ into the fp16 range folded into the BatchNorm scale, (2) a split-fp16 (hi + lo) 
 only.  This tool evaluates those and the other candidates with the format model of oracle/nn.py: every convolution of the
 tower is computed EXACTLY (fp64) on operands rounded the way a format would round them, everything else (folded BatchNorm,
 residual stream, heads) in fp32 -- so a row is the floor of what any kernel using that format can reach (tools/nn_diag.py
-shows that the tcgen05 kernel sits on its format's floor).
+shows that the tensor-core tower sits on its format's floor).
 
     fp16            both operands rounded to fp16 (what csrc/rz_net_tc2.cu does: 1 MMA per product)
     fp16-scaled     activations multiplied by a per-layer power of two that brings their maximum to 2^14 before rounding
