@@ -20,12 +20,17 @@
 //     shared-memory operand buffer.  The fp32 residual stream (the block inputs) does not fit beside
 //     the accumulators in the register file, nor beside the operands in shared memory; it goes to a
 //     per-CTA global scratch of the network (128 KB, written once and read once per block, L2-resident);
+//   * the epilogue does not wait on L2 one load at a time: a conv2 layer's first residual loads are issued before its
+//     last wgmma_wait and every later one kResAhead steps before its use; each layer's BN scale / shift is copied
+//     (cp.async) into the idle half of a double buffer while the previous layer's MMAs run; the 1x1 head-conv weights
+//     are staged in shared memory once per CTA;
 //   * the first conv (2 -> 256 channels, K = 18 padded to 32) is a 2-MMA GEMM on an im2col tile built
 //     from the two bitboards; the policy / value heads run on the math warps from the fp32 tower
 //     output.
 // HBM traffic per position: 16 B in, 260 B out.  Algorithmic work: 2 * 755,343,616 flop (SURVEY 3.2).
 #include <stdlib.h>
 #include <mutex>
+#include <type_traits>
 #include "rz_bitboard.cuh"
 #include "rz_net.cuh"
 #include "rz_tc_common.cuh"
@@ -42,14 +47,16 @@ constexpr int kMathThreads = 256;
 constexpr uint32_t kActCg = 2896, kActSlot = 144;
 constexpr uint32_t kActBytes = 32 * kActCg;  // 92,672
 constexpr uint32_t kStageBytes = 32768, kStages = 3;
+constexpr int kResAhead = 4;   // residual float4 loads a conv2 epilogue keeps in flight (16 registers; 8 would spill)
 constexpr uint32_t kA0Bytes = 8192, kW0Bytes = 16384;
 constexpr uint32_t kOffAct = 0;
 constexpr uint32_t kOffW = kOffAct + kActBytes;
 constexpr uint32_t kOffA0 = kOffW + kStages * kStageBytes;
 constexpr uint32_t kOffW0 = kOffA0 + kA0Bytes;
 constexpr uint32_t kOffSS = kOffW0 + kW0Bytes;           // 2 x [scale 256][shift 256] fp32
-constexpr uint32_t kOffPart = kOffSS + 2 * 2048;         // [2 halves][128 rows][4] fp32 head partial sums
-constexpr uint32_t kOffHp = kOffPart + 2 * 128 * 4 * 4;  // [2 boards][128]
+constexpr uint32_t kOffHw = kOffSS + 2 * 2048;           // 1x1 head-conv weights: policy [256][2], value [256] fp32
+constexpr uint32_t kOffPart = kOffHw + 768 * 4;          // [2 halves][128 rows][3] fp32 head partial sums
+constexpr uint32_t kOffHp = kOffPart + 2 * 128 * 3 * 4;  // [2 boards][128]
 constexpr uint32_t kOffHv = kOffHp + 2 * 128 * 4;        // [2][64]
 constexpr uint32_t kOffLogit = kOffHv + 2 * 64 * 4;      // [2][64]
 constexpr uint32_t kOffFc1 = kOffLogit + 2 * 64 * 4;     // [2][kTcMaxV]
@@ -86,6 +93,9 @@ __global__ void __launch_bounds__(kThreads, 1) net_tower_kernel(const Params pp)
     // ---- one-time setup -----------------------------------------------------------------------------
     for (uint32_t i = threadIdx.x * 16; i < kActBytes; i += kThreads * 16) *reinterpret_cast<uint4*>(sm + kOffAct + i) = make_uint4(0, 0, 0, 0);
     fence_proxy_async();
+    // the 1x1 head-conv weights are the same for every tile: staged once, read from shared memory by the last epilogue
+    for (uint32_t i = threadIdx.x; i < 768; i += kThreads)
+        reinterpret_cast<float*>(sm + kOffHw)[i] = __ldg(i < 512 ? p.blob + p.off_policy_conv + i : p.blob + p.off_value_conv + (i - 512));
     if (threadIdx.x == 0) {
         for (uint32_t s = 0; s < kStages; ++s) { mbar_init(bar_full(s), 1); mbar_init(bar_empty(s), 8 * CL); }
         mbar_init(bar_w0, 1);
@@ -141,10 +151,12 @@ __global__ void __launch_bounds__(kThreads, 1) net_tower_kernel(const Params pp)
         float* logit = reinterpret_cast<float*>(sm + kOffLogit);
         float* fc1 = reinterpret_cast<float*>(sm + kOffFc1);
         float4* res = reinterpret_cast<float4*>(p.res + (size_t)blockIdx.x * kTowerResFloatsPerCta) + et;   // + i * 256
-        const float* wpc = p.blob + p.off_policy_conv;
-        const float* wvc = p.blob + p.off_value_conv;
+        const float* hw = reinterpret_cast<const float*>(sm + kOffHw);
         uint32_t stage = 0, phase = 0, ss_buf = 0;
         float d[128];
+        // BN parameters of the first layer; every later layer's are fetched one layer ahead (below)
+        ss_s[et] = __ldg(p.ss + et);
+        ss_s[256 + et] = __ldg(p.ss + 256 + et);
 
         for (uint32_t it = 0; it < iters; ++it) {
             const uint32_t tile = blockIdx.x + it * gridDim.x;  // may be >= ntiles: dummy tile (no valid board)
@@ -158,12 +170,20 @@ __global__ void __launch_bounds__(kThreads, 1) net_tower_kernel(const Params pp)
             }
             float hs[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};   // head partial sums: (policy 0, policy 1, value) x (board 0, 1)
             for (int l = 0; l < L; ++l) {
-                // stage this layer's folded BN parameters (double-buffered across layers)
-                float* sc = ss_s + ss_buf * 512;
-                sc[et] = __ldg(p.ss + (size_t)l * 512 + et);
-                sc[256 + et] = __ldg(p.ss + (size_t)l * 512 + 256 + et);
-                ss_buf ^= 1;
-                epi_bar();   // operand (written by both warpgroups, made visible to the async proxy) and BN params ready
+                // folded BN parameters, double-buffered across layers: this layer's were copied in during the previous
+                // layer; the next layer's (after the last layer: the first layer's, for the next tile) are copied into
+                // the other buffer while this layer's MMAs run, so no layer starts on an L2 read
+                const float* sc = ss_s + ss_buf * 512;
+                const bool is_conv2 = l > 0 && (l & 1) == 0;   // second conv of a block: add the skip connection
+                float4 rb[kResAhead];   // residual loads in flight (conv2 layers)
+                epi_bar();   // operand (written by both warpgroups, made visible to the async proxy) and BN params ready;
+                             // every thread is done with layer l - 1's epilogue, so the other BN buffer is free
+                {
+                    const size_t nl = l + 1 < L ? (size_t)l + 1 : 0;
+                    const uint32_t dst = smem_u32(ss_s + (ss_buf ^ 1) * 512 + et);
+                    cp_async_4(dst, p.ss + nl * 512 + et);
+                    cp_async_4(dst + 1024, p.ss + nl * 512 + 256 + et);
+                }
                 acc_fence(d);
                 if (l == 0) {
                     mbar_wait(bar_w0, 0);
@@ -197,6 +217,11 @@ __global__ void __launch_bounds__(kThreads, 1) net_tower_kernel(const Params pp)
                             if (++stage == kStages) { stage = 0; phase ^= 1; }
                         }
                     }
+                    // the first residual loads of the epilogue overlap the last stage's MMAs
+                    if (is_conv2) {
+#pragma unroll
+                        for (int i = 0; i < kResAhead; ++i) rb[i] = res[i * 256];
+                    }
                     wgmma_wait<0>();
                     if (lane == 0) {
                         mbar_arrive(bar_empty(prev));
@@ -204,7 +229,8 @@ __global__ void __launch_bounds__(kThreads, 1) net_tower_kernel(const Params pp)
                     }
                 }
                 acc_fence(d);
-                const bool is_conv2 = l > 0 && (l & 1) == 0;   // second conv of a block: add the skip connection
+                cp_async_wait_all();   // the next layer's BN parameters have landed (published by the next barrier)
+                ss_buf ^= 1;
                 const bool keep_res = l == 0 || is_conv2;      // block output: keep an fp32 copy for the skip connection
                 const bool last = l == L - 1;
                 if (!last) epi_bar();   // both warpgroups' MMAs have finished reading the operand it is about to overwrite
@@ -214,6 +240,10 @@ __global__ void __launch_bounds__(kThreads, 1) net_tower_kernel(const Params pp)
                     if (pos0 < p.n) dbg0 = p.dbg_tower + ((size_t)pos0 * 64 + y * 8 + x) * 256;
                     if (pos0 + 1 < p.n) dbg1 = p.dbg_tower + ((size_t)(pos0 + 1) * 64 + y * 8 + x) * 256;
                 }
+                // the epilogue is compiled once with and once without the skip connection, so that a conv2 layer's
+                // residual loads land straight in the registers that consume them kResAhead steps later
+                auto epilogue = [&](auto conv2) {
+                    constexpr bool kConv2 = decltype(conv2)::value;
 #pragma unroll
                 for (int i = 0; i < 32; ++i) {
                     const int c = 8 * i + cq;
@@ -221,8 +251,9 @@ __global__ void __launch_bounds__(kThreads, 1) net_tower_kernel(const Params pp)
                     const float2 b = *reinterpret_cast<const float2*>(sc + 256 + c);
                     float v0 = fmaf(d[4 * i + 0], s.x, b.x), v1 = fmaf(d[4 * i + 1], s.y, b.y);
                     float v2 = fmaf(d[4 * i + 2], s.x, b.x), v3 = fmaf(d[4 * i + 3], s.y, b.y);
-                    if (is_conv2) {
-                        const float4 r = res[i * 256];
+                    if (kConv2) {   // step i's residual was loaded kResAhead steps earlier; its slot takes step i + kResAhead's
+                        const float4 r = rb[i % kResAhead];
+                        if (i + kResAhead < 32) rb[i % kResAhead] = res[(i + kResAhead) * 256];
                         v0 += r.x; v1 += r.y; v2 += r.z; v3 += r.w;
                     }
                     if (keep_res || last) {
@@ -237,19 +268,21 @@ __global__ void __launch_bounds__(kThreads, 1) net_tower_kernel(const Params pp)
                         asm volatile("st.shared.b32 [%0], %1;" ::"r"(act_row0 + off), "r"(h0) : "memory");
                         asm volatile("st.shared.b32 [%0], %1;" ::"r"(act_row1 + off), "r"(h1) : "memory");
                     } else {  // tower output feeds the 1x1 head convolutions (policy: 2 filters, value: 1)
-                        const float2 wa = __ldg(reinterpret_cast<const float2*>(wpc) + c);
-                        const float2 wb = __ldg(reinterpret_cast<const float2*>(wpc) + c + 1);
-                        const float va = __ldg(wvc + c), vb = __ldg(wvc + c + 1);
-                        hs[0] = fmaf(v1, wb.x, fmaf(v0, wa.x, hs[0]));
-                        hs[1] = fmaf(v1, wb.y, fmaf(v0, wa.y, hs[1]));
-                        hs[2] = fmaf(v1, vb, fmaf(v0, va, hs[2]));
-                        hs[3] = fmaf(v3, wb.x, fmaf(v2, wa.x, hs[3]));
-                        hs[4] = fmaf(v3, wb.y, fmaf(v2, wa.y, hs[4]));
-                        hs[5] = fmaf(v3, vb, fmaf(v2, va, hs[5]));
+                        const float4 w = *reinterpret_cast<const float4*>(hw + 2 * c);   // policy filters 0, 1 of c, c + 1
+                        const float2 wv = *reinterpret_cast<const float2*>(hw + 512 + c);
+                        hs[0] = fmaf(v1, w.z, fmaf(v0, w.x, hs[0]));
+                        hs[1] = fmaf(v1, w.w, fmaf(v0, w.y, hs[1]));
+                        hs[2] = fmaf(v1, wv.y, fmaf(v0, wv.x, hs[2]));
+                        hs[3] = fmaf(v3, w.z, fmaf(v2, w.x, hs[3]));
+                        hs[4] = fmaf(v3, w.w, fmaf(v2, w.y, hs[4]));
+                        hs[5] = fmaf(v3, wv.y, fmaf(v2, wv.x, hs[5]));
                         if (dbg0) *reinterpret_cast<float2*>(dbg0 + c) = make_float2(v0, v1);
                         if (dbg1) *reinterpret_cast<float2*>(dbg1 + c) = make_float2(v2, v3);
                     }
                 }
+                };
+                if (is_conv2) epilogue(std::true_type());
+                else epilogue(std::false_type());
                 if (!last) fence_proxy_async();
             }
             // ---- heads (agent/model.py:43-56) on the 256 math threads ----------------------------------

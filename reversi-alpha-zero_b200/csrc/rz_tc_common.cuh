@@ -66,6 +66,11 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
     asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
     return r;
 }
+// 4-byte global -> shared copy that needs no register (LDGSTS); cp_async_wait_all() waits for this thread's copies
+__device__ __forceinline__ void cp_async_4(uint32_t dst, const void* src) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(dst), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 // named barrier of the 256 math threads (warps 0..7)
 __device__ __forceinline__ void epi_bar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
@@ -171,20 +176,22 @@ __device__ __forceinline__ void build_layer0_operand(uint8_t* a0, u64 o, u64 e, 
 
 // heads (agent/model.py:43-56) on the 256 math threads of a CTA for its two boards: per-row partial sums of the 1x1 head
 // convolutions over two column halves (colhalf 0 / 1 of row m) -> BN + ReLU -> Dense(128 -> 64) + softmax,
-// Dense(64 -> V) + ReLU -> Dense(V -> 1) + tanh.  part [2][128][4], hp [2][128], hv [2][64], logit [2][64],
-// fc1 [2][kTcMaxV]: shared-memory scratch.
+// Dense(64 -> V) + ReLU -> Dense(V -> 1) + tanh.  part [2][128][3], hp [2][128], hv [2][64], logit [2][64],
+// fc1 [2][kTcMaxV]: shared-memory scratch.  The Dense loops are unrolled far enough that each thread's weight loads
+// (L2 hits: the shared-memory carve-out leaves L1 too small to keep them) go out in a few large batches; the
+// summation order stays the loop order.
 __device__ __forceinline__ void heads_phase(const Params& p, float hp0, float hp1, float hvv, int colhalf, int m, int brd, int y, int x,
                                             int et, int ew, int lane, uint32_t pos0, float* part, float* hp, float* hv, float* logit,
                                             float* fc1) {
     const float* ssh = p.ss + (size_t)p.n_layers * 512;
-    part[(colhalf * 128 + m) * 4 + 0] = hp0;
-    part[(colhalf * 128 + m) * 4 + 1] = hp1;
-    part[(colhalf * 128 + m) * 4 + 2] = hvv;
+    part[(colhalf * 128 + m) * 3 + 0] = hp0;
+    part[(colhalf * 128 + m) * 3 + 1] = hp1;
+    part[(colhalf * 128 + m) * 3 + 2] = hvv;
     epi_bar();
     if (colhalf == 0) {
-        const float a0 = part[m * 4 + 0] + part[(128 + m) * 4 + 0];
-        const float a1 = part[m * 4 + 1] + part[(128 + m) * 4 + 1];
-        const float av = part[m * 4 + 2] + part[(128 + m) * 4 + 2];
+        const float a0 = part[m * 3 + 0] + part[(128 + m) * 3 + 0];
+        const float a1 = part[m * 3 + 1] + part[(128 + m) * 3 + 1];
+        const float av = part[m * 3 + 2] + part[(128 + m) * 3 + 2];
         const int pix = y * 8 + x;
         hp[brd * 128 + pix] = fmaxf(fmaf(a0, ssh[0], ssh[2]), 0.f);        // Flatten is (C,H,W): index c*64 + pix
         hp[brd * 128 + 64 + pix] = fmaxf(fmaf(a1, ssh[1], ssh[3]), 0.f);
@@ -195,7 +202,7 @@ __device__ __forceinline__ void heads_phase(const Params& p, float hp0, float hp
         const int b = et >> 6, j = et & 63;
         const float* k = p.blob + p.off_policy_fc_k;
         float acc = __ldg(p.blob + p.off_policy_fc_b + j);
-#pragma unroll 8
+#pragma unroll 32
         for (int i = 0; i < 128; ++i) acc = fmaf(hp[b * 128 + i], __ldg(k + i * 64 + j), acc);
         logit[b * 64 + j] = acc;
     }
@@ -203,7 +210,7 @@ __device__ __forceinline__ void heads_phase(const Params& p, float hp0, float hp
         const int b = idx / p.V, j = idx - b * p.V;
         const float* k = p.blob + p.off_value_fc1_k;
         float acc = __ldg(p.blob + p.off_value_fc1_b + j);
-#pragma unroll 8
+#pragma unroll 32
         for (int i = 0; i < 64; ++i) acc = fmaf(hv[b * 64 + i], __ldg(k + (size_t)i * p.V + j), acc);
         fc1[b * kTcMaxV + j] = fmaxf(acc, 0.f);
     }
@@ -229,6 +236,7 @@ __device__ __forceinline__ void heads_phase(const Params& p, float hp0, float hp
     } else if (ew < 4) {  // value Dense(V -> 1) + tanh, one warp per board
         const int b = ew - 2;
         float acc = 0.f;
+#pragma unroll 16
         for (int j = lane; j < p.V; j += 32) acc = fmaf(fc1[b * kTcMaxV + j], __ldg(p.blob + p.off_value_fc2_k + j), acc);
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
