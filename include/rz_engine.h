@@ -337,6 +337,42 @@ int rz_ingest_dev(const rz_play_row* rows, size_t n_rows, int save_policy_of_tau
 int rz_ingest(const rz_play_row* rows, size_t n_rows, int save_policy_of_tau_1, int change_tau_turn,
               uint8_t* planes, float* policy, float* z);                       /* host pointers */
 
+/* ------------------------------------------------------------------------------------------------
+ * Trainer -- one SGD step of the network on the device (worker/optimize.py:73-86 OptimizeWorker.train_epoch ->
+ * Keras fit on agent/model.py:28-72,104-110).  Training-mode BatchNormalization (batch statistics, biased variance,
+ * epsilon 1e-3); loss = batch mean of sum -y log(p + 1e-7) + batch mean of (v - z)^2 + l2_reg * sum of squared Conv2D /
+ * Dense kernels; Keras SGD: v = momentum * v - lr * g, w = w + v for kernels, biases and BN gamma / beta; BN moving
+ * statistics: moving = bn_momentum * moving + (1 - bn_momentum) * batch statistic.  3x3 convolutions use TF32 operands
+ * with fp32 accumulation; every reduction has a fixed order, so equal inputs give bit-identical weights.
+ * Configurations: filters a multiple of 16 in [16, 256], kernel_size 3, any res_blocks and value_fc (else RZ_EINVAL).
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct rz_trainer rz_trainer;
+
+typedef struct rz_train_cfg {
+    int32_t max_batch;  /* largest batch rz_trainer_step_dev will be given (sizes the saved activations) */
+    float momentum;     /* SGD(momentum=0.9), worker/optimize.py:84 */
+    float l2_reg;       /* ModelConfig.l2_reg (config.py:192) */
+    float bn_momentum;  /* Keras BatchNormalization momentum, 0.99 */
+} rz_train_cfg;
+
+int rz_trainer_create(const rz_net_cfg* net, const rz_train_cfg* cfg, int device, rz_trainer** out);
+int rz_trainer_destroy(rz_trainer* t);
+/* same count as rz_net_blob_size for the same configuration */
+int rz_trainer_blob_size(const rz_trainer* t, size_t* n_floats);
+/* weights in the blob layout of rz_net_load_weights; both also zero the momentum */
+int rz_trainer_load_weights(rz_trainer* t, const float* blob_host, size_t n_floats);
+int rz_trainer_load_weights_dev(rz_trainer* t, const float* blob_dev, size_t n_floats, void* stream);
+/* current weights, blob layout (ready for rz_net_load_weights_dev or a model_weight.rzblob.npy file) */
+int rz_trainer_weights_dev(rz_trainer* t, float* blob_dev, size_t n_floats, void* stream);
+/* one step on records index[0..batch) of the device arrays planes[n_records][2][8][8] u8, policy[n_records][64] f32,
+ * z[n_records] f32 (what rz_ingest_dev writes); 1 <= batch <= max_batch; indices may repeat.  loss_dev[3] (device) =
+ * total, policy, value loss of the batch before the update.  Asynchronous: no host synchronisation.  An index outside
+ * [0, n_records) is never read: the step then leaves the weights unchanged and writes NaN losses. */
+int rz_trainer_step_dev(rz_trainer* t, const uint8_t* planes, const float* policy, const float* z, size_t n_records,
+                        const int32_t* index, size_t batch, float lr, float* loss_dev, void* stream);
+/* test hook: gradient of the last step's total loss in blob layout (0 in the moving-statistics slots) */
+int rz_trainer_last_grad_dev(rz_trainer* t, float* grad_dev, size_t n_floats, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -27,6 +27,10 @@ class NetCfg(C.Structure):
     _fields_ = [("filters", C.c_int32), ("res_blocks", C.c_int32), ("value_fc", C.c_int32), ("kernel_size", C.c_int32)]
 
 
+class TrainCfg(C.Structure):
+    _fields_ = [("max_batch", C.c_int32), ("momentum", C.c_float), ("l2_reg", C.c_float), ("bn_momentum", C.c_float)]
+
+
 class EngineCfg(C.Structure):
     _fields_ = [(n, C.c_int32) for n in (
         "games", "simulation_num_per_move", "parallel_search_num", "virtual_loss", "change_tau_turn", "thinking_loop",
@@ -107,6 +111,14 @@ SIGNATURES = {
     "rz_read_play_rows": (C.c_int, [C.c_char_p, vp, sz, C.POINTER(sz), C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "rz_ingest_dev": (C.c_int, [vp, sz, C.c_int, C.c_int, vp, vp, vp, vp]),
     "rz_ingest": (C.c_int, [vp, sz, C.c_int, C.c_int, u8p, f32p, f32p]),
+    "rz_trainer_create": (C.c_int, [C.POINTER(NetCfg), C.POINTER(TrainCfg), C.c_int, C.POINTER(vp)]),
+    "rz_trainer_destroy": (C.c_int, [vp]),
+    "rz_trainer_blob_size": (C.c_int, [vp, C.POINTER(sz)]),
+    "rz_trainer_load_weights": (C.c_int, [vp, f32p, sz]),
+    "rz_trainer_load_weights_dev": (C.c_int, [vp, vp, sz, vp]),
+    "rz_trainer_weights_dev": (C.c_int, [vp, vp, sz, vp]),
+    "rz_trainer_step_dev": (C.c_int, [vp, vp, vp, vp, sz, vp, sz, C.c_float, vp, vp]),
+    "rz_trainer_last_grad_dev": (C.c_int, [vp, vp, sz, vp]),
 }
 
 _lib = None

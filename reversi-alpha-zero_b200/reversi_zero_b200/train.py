@@ -1,0 +1,97 @@
+"""Handle of the device trainer (rz_trainer_* in include/rz_engine.h): one SGD step of the policy/value network per call
+on a device-resident dataset (what ``worker.ingest.to_training_tensors`` returns), in the reference's Keras semantics
+(worker/optimize.py:73-86, agent/model.py:28-72,104-110).  The weights exchanged are the float32 blob ``Net`` loads.
+
+    tr = Trainer(model_config, max_batch=256)
+    tr.load_blob(blob)
+    loss = tr.step(states, policy, z, index, lr)   # index: int32 CUDA tensor of record numbers (a slice of a permutation)
+    net.load_blob_dev(tr.blob_dev())
+"""
+import ctypes as C
+
+import numpy as np
+
+from . import _cabi
+from .agent import model as M
+
+MOMENTUM = 0.9      # SGD(momentum=0.9), worker/optimize.py:84
+BN_MOMENTUM = 0.99  # Keras BatchNormalization default
+
+
+class Trainer:
+    def __init__(self, model_config, max_batch, device=0, momentum=MOMENTUM, bn_momentum=BN_MOMENTUM, l2_reg=None):
+        import torch
+        self.mc = model_config
+        self.device = torch.device("cuda", device)
+        self.max_batch = int(max_batch)
+        self._h = C.c_void_p()
+        ncfg = _cabi.NetCfg(model_config.cnn_filter_num, model_config.res_layer_num, model_config.value_fc_size,
+                            model_config.cnn_filter_size)
+        tcfg = _cabi.TrainCfg(self.max_batch, momentum, model_config.l2_reg if l2_reg is None else l2_reg, bn_momentum)
+        _cabi.check(_cabi.lib().rz_trainer_create(C.byref(ncfg), C.byref(tcfg), device, C.byref(self._h)), "rz_trainer_create")
+        n = C.c_size_t()
+        _cabi.check(_cabi.lib().rz_trainer_blob_size(self._h, C.byref(n)), "rz_trainer_blob_size")
+        self.blob_floats = n.value
+        assert self.blob_floats == M.blob_size(model_config)
+
+    def _stream(self):
+        import torch
+        return torch.cuda.current_stream(self.device).cuda_stream
+
+    def load_blob(self, blob):
+        """host float32 blob; also zeroes the momentum"""
+        blob = np.ascontiguousarray(blob, dtype=np.float32)
+        _cabi.check(_cabi.lib().rz_trainer_load_weights(self._h, blob.ctypes.data_as(_cabi.f32p), blob.size), "rz_trainer_load_weights")
+
+    def load_blob_dev(self, tensor):
+        """float32 CUDA tensor holding the blob; also zeroes the momentum"""
+        _cabi.check(_cabi.lib().rz_trainer_load_weights_dev(self._h, C.c_void_p(tensor.data_ptr()), tensor.numel(), self._stream()),
+                    "rz_trainer_load_weights_dev")
+
+    def blob_dev(self):
+        """current weights as a float32 CUDA tensor (blob layout)"""
+        import torch
+        out = torch.empty(self.blob_floats, dtype=torch.float32, device=self.device)
+        _cabi.check(_cabi.lib().rz_trainer_weights_dev(self._h, C.c_void_p(out.data_ptr()), out.numel(), self._stream()),
+                    "rz_trainer_weights_dev")
+        return out
+
+    def blob(self):
+        return self.blob_dev().cpu().numpy()
+
+    def step(self, states, policy, z, index, lr):
+        """One step on records ``index`` of (states uint8 [N,2,8,8], policy float32 [N,64], z float32 [N]), all CUDA tensors.
+        Returns a new device tensor [total, policy, value] with this batch's loss (NaN and no update if an index is out of
+        range); reading it is the only synchronisation."""
+        import torch
+        for t, dt in ((states, torch.uint8), (policy, torch.float32), (z, torch.float32), (index, torch.int32)):
+            if t.dtype != dt or not t.is_cuda or not t.is_contiguous():
+                raise ValueError(f"expected a contiguous CUDA tensor of {dt}, got {t.dtype} on {t.device}")
+        n = states.shape[0]
+        if policy.shape != (n, 64) or z.shape != (n,) or tuple(states.shape[1:]) != (2, 8, 8) or index.dim() != 1:
+            raise ValueError("expected states [N,2,8,8], policy [N,64], z [N], index [B]")
+        loss = torch.empty(3, dtype=torch.float32, device=self.device)
+        _cabi.check(_cabi.lib().rz_trainer_step_dev(self._h, C.c_void_p(states.data_ptr()), C.c_void_p(policy.data_ptr()),
+                                                     C.c_void_p(z.data_ptr()), n, C.c_void_p(index.data_ptr()), index.numel(),
+                                                     float(lr), C.c_void_p(loss.data_ptr()), self._stream()),
+                    "rz_trainer_step_dev")
+        return loss
+
+    def last_grad(self):
+        """gradient of the last step's total loss, host float32 blob layout (0 in the moving-statistics slots)"""
+        import torch
+        out = torch.empty(self.blob_floats, dtype=torch.float32, device=self.device)
+        _cabi.check(_cabi.lib().rz_trainer_last_grad_dev(self._h, C.c_void_p(out.data_ptr()), out.numel(), self._stream()),
+                    "rz_trainer_last_grad_dev")
+        return out.cpu().numpy()
+
+    def close(self):
+        if self._h:
+            _cabi.lib().rz_trainer_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass

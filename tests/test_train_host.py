@@ -1,0 +1,110 @@
+"""CPU suite for the device trainer: the fp64 oracle step (oracle/train.py) against central finite differences and a
+hand computation of the Keras update rules, the TF32 format model, and the trainer's configuration checks (which run
+before any CUDA call)."""
+import ctypes as C
+
+import numpy as np
+import pytest
+import torch
+import torch.nn.functional as F
+
+from oracle import nn as onn, train as ot
+from reversi_zero_b200 import _cabi
+from reversi_zero_b200.agent import model as M
+
+MINI = dict(cnn_filter_num=16, res_layer_num=1, value_fc_size=8)
+
+
+def _batch(n, seed):
+    rng = np.random.default_rng(seed)
+    a = rng.integers(0, 2 ** 64, n, dtype=np.uint64)
+    r = rng.integers(0, 2 ** 64, n, dtype=np.uint64)
+    planes = onn.planes_from_bitboards(a & r, a & ~r)
+    policy = rng.dirichlet(np.full(64, 0.3), n).astype(np.float32)
+    z = rng.choice([-1.0, 0.0, 1.0], n).astype(np.float32)
+    return planes, policy, z
+
+
+def _weights(mc, seed):
+    w = M.build_random_weights(mc, seed, perturb_bn=True)
+    return {k: v.astype(np.float64) for k, v in w.items()}
+
+
+def test_oracle_gradient_matches_central_differences():
+    mc = M.ModelConfig(**MINI)
+    w = _weights(mc, 1)
+    planes, policy, z = _batch(4, 2)
+    l2 = 1e-4
+    (total, _, _), grads, _ = ot.loss_and_grad(w, planes, policy, z, 1, l2)
+
+    def loss_at(ww):
+        return ot.loss_and_grad(ww, planes, policy, z, 1, l2)[0][0]
+
+    rng = np.random.default_rng(3)
+    h = 1e-6  # small enough that no ReLU input of the 4 x 64 pixels changes sign inside the stencil
+    for name, g in grads.items():
+        for _ in range(2):  # random unit directions: every element of the tensor takes part
+            d = rng.standard_normal(g.shape)
+            d /= np.linalg.norm(d)
+            wp, wm = dict(w), dict(w)
+            wp[name] = w[name] + h * d
+            wm[name] = w[name] - h * d
+            fd = (loss_at(wp) - loss_at(wm)) / (2 * h)
+            an = float((g * d).sum())
+            if name.endswith(".bias") and not name.startswith(("policy_fc", "value_fc")):
+                assert abs(fd) < 1e-8 and abs(an) < 1e-12, (name, fd, an)  # conv bias under training-mode BN: exactly 0
+            else:
+                assert abs(fd - an) <= 1e-6 * abs(an) + 1e-12, (name, fd, an)
+
+
+def test_oracle_moving_statistics_and_keras_sgd_by_hand():
+    mc = M.ModelConfig(**MINI)
+    w = _weights(mc, 4)
+    planes, policy, z = _batch(6, 5)
+    w1, v1, _, g1 = ot.step(w, None, planes, policy, z, 0.1, 1, 1e-4)
+    # conv0's batch statistics by hand
+    k = torch.from_numpy(w["conv0.kernel"]).permute(3, 2, 0, 1)
+    y = F.conv2d(torch.from_numpy(planes).double(), k, torch.from_numpy(w["conv0.bias"]), padding=1).numpy()
+    mean, var = y.mean(axis=(0, 2, 3)), y.var(axis=(0, 2, 3))
+    np.testing.assert_allclose(w1["conv0.bn_mean"], 0.99 * w["conv0.bn_mean"] + 0.01 * mean, rtol=1e-12, atol=1e-14)
+    np.testing.assert_allclose(w1["conv0.bn_var"], 0.99 * w["conv0.bn_var"] + 0.01 * var, rtol=1e-12, atol=1e-14)
+    # Keras SGD with an lr change: v = 0.9 v - lr g; w = w + v (not torch.optim.SGD's v = 0.9 v + g; w -= lr v)
+    w2, v2, _, g2 = ot.step(w1, v1, planes, policy, z, 0.01, 1, 1e-4)
+    for name in g1:
+        np.testing.assert_allclose(v1[name], -0.1 * g1[name], rtol=1e-12, atol=1e-15)
+        np.testing.assert_allclose(w2[name], w[name] - 0.1 * g1[name] + 0.9 * (-0.1 * g1[name]) - 0.01 * g2[name], rtol=1e-10,
+                                   atol=1e-13)
+    torch_sgd = w1["policy_fc.kernel"] - 0.01 * (0.9 * g1["policy_fc.kernel"] + g2["policy_fc.kernel"])
+    assert np.abs(torch_sgd - w2["policy_fc.kernel"]).max() > 1e-4  # the two forms really differ after an lr change
+    # the L2 term counts kernels only and is not divided by the batch size
+    wk = dict(w)
+    wk["policy_fc.bias"] = w["policy_fc.bias"] + 1.0
+    l_a = ot.loss_and_grad(w, planes, policy, z, 1, 0.5)[0]
+    l_b = ot.loss_and_grad(w, planes, policy, z, 1, 0.0)[0]
+    expected = 0.5 * sum((v ** 2).sum() for n, v in w.items() if n.endswith(".kernel"))
+    assert abs((l_a[0] - l_b[0]) - expected) < 1e-9 * expected
+
+
+def test_tf32_rounding_and_format_model():
+    x = torch.tensor([1.0, 1.0 + 2 ** -11, 1.0 + 2 ** -10, -(1.0 + 2 ** -11), 3.0e-3, 0.0], dtype=torch.float64)
+    r = ot.tf32(x)
+    assert r[0] == 1.0 and r[1] == 1.0 + 2 ** -10 and r[2] == 1.0 + 2 ** -10 and r[3] == -(1.0 + 2 ** -10) and r[5] == 0.0
+    assert (ot.tf32(r) == r).all()
+    mc = M.ModelConfig(**MINI)
+    w = _weights(mc, 6)
+    planes, policy, z = _batch(8, 7)
+    l64, g64, _ = ot.loss_and_grad(w, planes, policy, z, 1, 1e-4)
+    lfm, gfm, _ = ot.loss_and_grad(w, planes, policy, z, 1, 1e-4, tf32_convs=True)
+    assert abs(lfm[0] - l64[0]) < 1e-3 * abs(l64[0])
+    for k in ("res0.conv1.kernel", "conv0.kernel", "policy_fc.kernel"):
+        err = np.linalg.norm(gfm[k] - g64[k]) / np.linalg.norm(g64[k])
+        assert 0 < err < 5e-2, (k, err)  # TF32's 2^-11 unit roundoff, amplified by the BN backward's cancellation
+
+
+@pytest.mark.parametrize("filters,res,kernel,batch", [(24, 1, 3, 8), (8, 1, 3, 8), (272, 1, 3, 8), (16, 1, 5, 8), (16, 1, 3, 0)])
+def test_trainer_rejects_unsupported_configurations(filters, res, kernel, batch):
+    ncfg = _cabi.NetCfg(filters, res, 8, kernel)
+    tcfg = _cabi.TrainCfg(batch, 0.9, 1e-4, 0.99)
+    h = C.c_void_p()
+    assert _cabi.lib().rz_trainer_create(C.byref(ncfg), C.byref(tcfg), 0, C.byref(h)) == -1  # RZ_EINVAL
+    assert not h.value
