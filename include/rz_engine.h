@@ -113,6 +113,8 @@ typedef struct rz_net_cfg {
 #define RZ_NET_IMPL_AUTO 0    /* wgmma tower when filters == 256, else the generic kernel */
 #define RZ_NET_IMPL_GENERIC 1 /* CUDA-core fp32 kernel, any configuration */
 #define RZ_NET_IMPL_TCGEN05 2 /* fused persistent tensor-core (wgmma) tower (filters must be 256) */
+#define RZ_NET_IMPL_SPLIT 3   /* the same tower with each 2-board tile split over an 8-CTA cluster: lower latency for small
+                                 batches, bit-identical outputs (filters must be 256); AUTO picks it up to a measured batch size */
 
 /* Thread-block clusters of the tensor-core tower from now on (process-wide): 2 = CTA pairs that share every weight stage
  * through cluster multicast (default; falls back to 1 where the GPU cannot hold a pair), 1 = single CTAs.  The default
@@ -144,6 +146,11 @@ int rz_net_debug_tower_dev(rz_net* net, const uint64_t* own, const uint64_t* ene
  * ("policy/value logits within 1e-3") can be asserted on the logits themselves; tower may be NULL. */
 int rz_net_debug_heads_dev(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value,
                            float* tower, float* policy_logits, float* value_logit, size_t n, void* stream);
+/* same, with the tower implementation chosen: RZ_NET_IMPL_AUTO, _TCGEN05 or _SPLIT. */
+int rz_net_debug_heads_impl_dev(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value,
+                                float* tower, float* policy_logits, float* value_logit, size_t n, int impl, void* stream);
+/* the implementation RZ_NET_IMPL_AUTO runs for a batch of n positions (on the engine's counted path: its capacity). */
+int rz_net_select_impl(const rz_net* net, size_t n, int* impl);
 /* ReversiModelAPI.predict (agent/api.py:30-45): planes uint8 [n][2][8][8] with values {0,1}, host
  * buffers in, policy[n][64] / value[n] host buffers out. */
 int rz_net_predict(rz_net* net, const uint8_t* planes, float* policy, float* value, size_t n, int impl);

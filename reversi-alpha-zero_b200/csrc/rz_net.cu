@@ -176,14 +176,26 @@ int net_forward_generic(rz_net* net, const uint64_t* own, const uint64_t* enemy,
     return RZ_OK;
 }
 
+// Largest batch (capacity) for which AUTO runs the split tower; both towers compute the same bits.  0: on a 400 W H100
+// 80GB HBM3 the split tower was not faster at any batch (ch5, n = 1..16: 0.50 ms vs 0.49-0.50 ms per launch; n = 32:
+// 0.99 vs 0.50 ms), tools/search_latency_bench.py, DESIGN.md §5 "Split tower".
+constexpr size_t kSplitMaxBatch = 0;
+
+int select_impl(const rz_net* net, size_t n, int impl) {
+    if (impl != RZ_NET_IMPL_AUTO) return impl;
+    if (net->cfg.filters != 256) return RZ_NET_IMPL_GENERIC;
+    return n <= kSplitMaxBatch ? RZ_NET_IMPL_SPLIT : RZ_NET_IMPL_TCGEN05;
+}
+
 int net_forward(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value, size_t n, int impl,
                 cudaStream_t stream) {
     if (!net->loaded) { set_error("rz_net: weights not loaded"); return RZ_ESTATE; }
     if (n == 0) return RZ_OK;
-    if (impl == RZ_NET_IMPL_AUTO) impl = net->cfg.filters == 256 ? RZ_NET_IMPL_TCGEN05 : RZ_NET_IMPL_GENERIC;
-    if (impl == RZ_NET_IMPL_TCGEN05) {
-        RZ_REQUIRE(net->cfg.filters == 256, "wgmma tower requires filters == 256 (got %d)", net->cfg.filters);
-        return net_forward_tc(net, own, enemy, policy, value, n, stream, nullptr);
+    impl = select_impl(net, n, impl);
+    if (impl == RZ_NET_IMPL_TCGEN05 || impl == RZ_NET_IMPL_SPLIT) {
+        RZ_REQUIRE(net->cfg.filters == 256, "tensor-core towers require filters == 256 (got %d)", net->cfg.filters);
+        return impl == RZ_NET_IMPL_SPLIT ? net_forward_split(net, own, enemy, policy, value, n, stream, nullptr)
+                                         : net_forward_tc(net, own, enemy, policy, value, n, stream, nullptr);
     }
     RZ_REQUIRE(impl == RZ_NET_IMPL_GENERIC, "unknown net impl %d", impl);
     return net_forward_generic(net, own, enemy, policy, value, n, stream);
@@ -192,8 +204,9 @@ int net_forward(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* 
 int net_forward_counted(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value,
                         const uint32_t* count_dev, size_t max_n, int impl, cudaStream_t stream) {
     if (!net->loaded) { set_error("rz_net: weights not loaded"); return RZ_ESTATE; }
-    if (impl == RZ_NET_IMPL_AUTO) impl = net->cfg.filters == 256 ? RZ_NET_IMPL_TCGEN05 : RZ_NET_IMPL_GENERIC;
+    impl = select_impl(net, max_n, impl);
     if (impl == RZ_NET_IMPL_TCGEN05) return net_forward_tc(net, own, enemy, policy, value, max_n, stream, nullptr, count_dev);
+    if (impl == RZ_NET_IMPL_SPLIT) return net_forward_split(net, own, enemy, policy, value, max_n, stream, nullptr, count_dev);
     return net_forward_generic(net, own, enemy, policy, value, max_n, stream, count_dev);
 }
 
@@ -317,6 +330,25 @@ int rz_net_debug_heads_dev(rz_net* net, const uint64_t* own, const uint64_t* ene
     RZ_REQUIRE(net && own && enemy && policy && value && policy_logits && value_logit, "rz_net_debug_heads_dev: null pointer");
     if (!net->loaded) { set_error("rz_net: weights not loaded"); return RZ_ESTATE; }
     return net_forward_tc(net, own, enemy, policy, value, n, (cudaStream_t)stream, tower, nullptr, policy_logits, value_logit);
+}
+
+int rz_net_debug_heads_impl_dev(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value, float* tower,
+                                float* policy_logits, float* value_logit, size_t n, int impl, void* stream) {
+    RZ_REQUIRE(net && own && enemy && policy && value && policy_logits && value_logit, "rz_net_debug_heads_impl_dev: null pointer");
+    if (!net->loaded) { set_error("rz_net: weights not loaded"); return RZ_ESTATE; }
+    RZ_REQUIRE(net->cfg.filters == 256, "tensor-core towers require filters == 256 (got %d)", net->cfg.filters);
+    if (n == 0) return RZ_OK;
+    impl = select_impl(net, n, impl);
+    if (impl == RZ_NET_IMPL_SPLIT)
+        return net_forward_split(net, own, enemy, policy, value, n, (cudaStream_t)stream, tower, nullptr, policy_logits, value_logit);
+    RZ_REQUIRE(impl == RZ_NET_IMPL_TCGEN05, "rz_net_debug_heads_impl_dev: impl must be AUTO, TCGEN05 or SPLIT (got %d)", impl);
+    return net_forward_tc(net, own, enemy, policy, value, n, (cudaStream_t)stream, tower, nullptr, policy_logits, value_logit);
+}
+
+int rz_net_select_impl(const rz_net* net, size_t n, int* impl) {
+    RZ_REQUIRE(net && impl, "rz_net_select_impl: null pointer");
+    *impl = select_impl(net, n, RZ_NET_IMPL_AUTO);
+    return RZ_OK;
 }
 
 int rz_net_predict(rz_net* net, const uint8_t* planes, float* policy, float* value, size_t n, int impl) {

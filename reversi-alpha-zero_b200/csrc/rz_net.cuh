@@ -50,6 +50,12 @@ int net_forward_tc(rz_net* net, const uint64_t* own, const uint64_t* enemy, floa
                    cudaStream_t stream, float* dbg_tower /* nullable: [n][64][256] fp32 tower output */,
                    const uint32_t* n_dev = nullptr /* nullable: actual batch size in device memory (<= n) */,
                    float* dbg_logits = nullptr /* nullable: [n][64] policy logits */, float* dbg_vlogit = nullptr /* nullable: [n] */);
+// same function as net_forward_tc, bit for bit, one 8-CTA cluster per 2-board tile (small batches, rz_net_split.cu)
+int net_forward_split(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value, size_t n,
+                      cudaStream_t stream, float* dbg_tower, const uint32_t* n_dev = nullptr, float* dbg_logits = nullptr,
+                      float* dbg_vlogit = nullptr);
+// RZ_NET_IMPL_AUTO -> the implementation used for a batch of capacity n
+int select_impl(const rz_net* net, size_t n, int impl);
 int net_pack_tc(rz_net* net, cudaStream_t stream);
 // thread-block clusters of the tower kernel: 2 = CTA pairs sharing the weight stages (default), 1 = single CTAs
 int set_tower_cluster(int cluster);

@@ -94,6 +94,8 @@ SIGNATURES = {
     "rz_net_set_tower_cluster": (C.c_int, [C.c_int]),
     "rz_net_debug_tower_dev": (C.c_int, [vp, vp, vp, vp, vp, vp, sz, vp]),
     "rz_net_debug_heads_dev": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, vp, sz, vp]),
+    "rz_net_debug_heads_impl_dev": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, vp, sz, C.c_int, vp]),
+    "rz_net_select_impl": (C.c_int, [vp, sz, C.POINTER(C.c_int)]),
     "rz_net_predict": (C.c_int, [vp, u8p, f32p, f32p, sz, C.c_int]),
     "rz_engine_create": (C.c_int, [C.POINTER(EngineCfg), vp, C.c_int, C.POINTER(vp)]),
     "rz_engine_destroy": (C.c_int, [vp]),

@@ -43,6 +43,7 @@ class ReversiPlayer:
         for k in ("use_solver_turn_in_simulation", "virtual_loss"):
             if hasattr(self.config.play, k):
                 setattr(search_pc, k, getattr(self.config.play, k))
+        search_pc.thinking_loop = max(1, int(search_pc.thinking_loop))   # the loop runs on the host (below); see there
         ecfg = engine_cfg_from_play_config(search_pc, games=1, seed=seed,
                                            eval_mode=EVAL_NET if model is not None else EVAL_FAKE)
         self.engine = Engine(ecfg, model, device)
@@ -67,13 +68,14 @@ class ReversiPlayer:
     def _search(self, own, enemy):
         """simulation_num_per_move simulations from (own, enemy); with a CallbackInMCTS the search runs in chunks of
         `per_sim` simulations (the tree is kept between chunks) and reports (q, n) after each, like
-        agent/player.py:212-214; stop_thinking() ends it early (:206-208)."""
+        agent/player.py:212-214; stop_thinking() ends it early (:206-208).  The reference reports whenever the number of
+        simulations still to finish is a multiple of `per_sim`, so a remainder comes first: 25 in chunks of 10 -> 5, 10, 10."""
         total = int(self.play_config.simulation_num_per_move)
         cb = self.callback_in_mtcs
         chunk = int(cb.per_sim) if cb and cb.per_sim > 0 else total
         done, n, w = 0, None, None
         while done < total and not (self.requested_stop_thinking and done > 0):
-            step = min(chunk, total - done)
+            step = (total - done) % chunk or chunk
             if step != self._engine_sims:
                 self.engine.set_simulation_num(step)
                 self._engine_sims = step
@@ -99,10 +101,15 @@ class ReversiPlayer:
             if mv is not None:
                 policy = np.zeros(64)
                 policy[mv] = 1
-                self.thinking_history[(own, enemy)] = HistoryItem(mv, policy, None, None, None, None)
+                # :157-160: N = 999 and W = sign(score) * 999 on the solved move
+                n, w = np.zeros(64), np.zeros(64)
+                n[mv], w[mv] = 999, np.sign(score) * 999
+                self.thinking_history[(own, enemy)] = HistoryItem(mv, policy, list(w / (n + 1e-5)), list(n), None, None)
                 return ActionWithEvaluation(action=mv, n=999, q=float(np.sign(score)))  # not saved as play data
         n = w = None
-        for tl in range(pc.thinking_loop):
+        # at least one search: NBoard's `set depth` can make thinking_loop 0 (e.g. depth 1 at 200 simulations per move),
+        # where the reference fails with an unbound `action`
+        for tl in range(max(1, pc.thinking_loop)):
             if turn > 0:
                 n, w = self._search(own, enemy)
             else:  # bypass_first_move, agent/player.py:143-148

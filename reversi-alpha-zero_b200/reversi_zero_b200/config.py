@@ -1,6 +1,6 @@
 """Configuration tree with the reference's field names and defaults (config.py:15-193) so that the
 reference's YAML files (config/*.yml) and its own ``Config`` objects drive the H100 engine unchanged.
-Only the sections the self-play path reads are modelled; any object exposing the same attributes
+Only the sections the self-play path and the NBoard engine read are modelled; any object exposing the same attributes
 (e.g. the reference's ``Config`` built by moke_config) is accepted everywhere in this package.
 
 Engine-specific knobs live in ``Config.b200`` (not present in the reference): concurrent games per
@@ -90,6 +90,34 @@ class PlayConfig(_Section):
         self.schedule_of_simulation_num_per_move = [(0, 8), (300, 50), (2000, 200)]
 
 
+class PlayWithHumanConfig(_Section):
+    """Search settings for games against a person or another engine, config.py:74-92"""
+
+    def __init__(self):
+        self.parallel_search_num = 8
+        self.noise_eps = 0
+        self.change_tau_turn = 0
+        self.resign_threshold = None
+        self.use_newest_next_generation_model = True
+
+    def update_play_config(self, pc):
+        pc.noise_eps = self.noise_eps
+        pc.change_tau_turn = self.change_tau_turn
+        pc.parallel_search_num = self.parallel_search_num
+        pc.resign_threshold = self.resign_threshold
+        pc.use_newest_next_generation_model = self.use_newest_next_generation_model
+
+
+class NBoardConfig(_Section):
+    """NBoard engine, config.py:95-100"""
+
+    def __init__(self):
+        self.my_name = "RAZ"
+        self.read_stdin_timeout = 0.1
+        self.simulation_num_per_depth_about = 20
+        self.hint_callback_per_sim = 10
+
+
 class B200Config(_Section):
     """Engine knobs that have no counterpart in the reference."""
 
@@ -112,6 +140,8 @@ class Config(_Section):
         self.model = ModelConfig()
         self.play = PlayConfig()
         self.play_data = PlayDataConfig()
+        self.play_with_human = PlayWithHumanConfig()
+        self.nboard = NBoardConfig()
         self.b200 = B200Config()
 
 

@@ -1,5 +1,48 @@
-"""GGF move text / game record formatting used by the self-play worker (reference lib/ggf.py:56-100)."""
+"""GGF game records (reference lib/ggf.py): parsing for the NBoard engine, move text and record formatting for the
+self-play worker."""
+import re
+from collections import namedtuple
 from datetime import datetime, timezone
+
+GGF = namedtuple("GGF", "BO MOVES")
+BO = namedtuple("BO", "board_type, square_cont, color")  # color: {O, *}  (O is white, * is black)
+MOVE = namedtuple("MOVE", "color pos")  # color={B, W} pos: like 'F5'
+
+_TAG = re.compile(r'([a-zA-Z]+)\[([^\]]+)\]')
+
+
+def parse_ggf(ggf):
+    """lib/ggf.py:13-32: the board (BO) and the moves (B / W) of a GGF game; every other tag is ignored."""
+    moves = []
+    bo = None
+    for token in re.split(r'([a-zA-Z]+\[[^\]]+\])', ggf):
+        match = _TAG.search(token)
+        if not match:
+            continue
+        key, value = match.groups()
+        key = key.upper()
+        if key == "BO":
+            bo = BO(*value.split(" "))
+        elif key in ("B", "W"):
+            moves.append(MOVE(key, value))
+    return GGF(bo, moves)
+
+
+def parse_ggf_board_to_bitboard(string):
+    """lib/util.py:22-29: '*' = black, 'O' = white, square i = bit i."""
+    white = black = 0
+    for i, ch in enumerate(string):
+        if ch == "*":
+            black |= 1 << i
+        elif ch == "O":
+            white |= 1 << i
+    return black, white
+
+
+def convert_to_bitboard_and_actions(ggf):
+    """lib/ggf.py:62-67 -> (black, white, [action or None for a pass])"""
+    black, white = parse_ggf_board_to_bitboard(ggf.BO.square_cont)
+    return black, white, [convert_move_to_action(move.pos) for move in ggf.MOVES]
 
 
 def convert_action_to_move(action):

@@ -6,7 +6,7 @@ import numpy as np
 from . import _cabi
 from .agent import model as M
 
-IMPL_AUTO, IMPL_GENERIC, IMPL_TCGEN05 = 0, 1, 2
+IMPL_AUTO, IMPL_GENERIC, IMPL_TCGEN05, IMPL_SPLIT = 0, 1, 2, 3
 
 
 def set_tower_cluster(cluster):
@@ -73,6 +73,19 @@ class Net:
                                                         C.c_void_p(tower_t.data_ptr()) if tower_t is not None else None,
                                                         C.c_void_p(logits_t.data_ptr()), C.c_void_p(vlogit_t.data_ptr()), n, stream_ptr),
                     "rz_net_debug_heads_dev")
+
+    def debug_heads_impl_dev(self, own_t, enemy_t, policy_t, value_t, logits_t, vlogit_t, n, impl, tower_t=None, stream_ptr=None):
+        """debug_heads_dev with the tower implementation chosen (IMPL_AUTO, IMPL_TCGEN05 or IMPL_SPLIT)"""
+        _cabi.check(_cabi.lib().rz_net_debug_heads_impl_dev(
+            self._h, C.c_void_p(own_t.data_ptr()), C.c_void_p(enemy_t.data_ptr()), C.c_void_p(policy_t.data_ptr()),
+            C.c_void_p(value_t.data_ptr()), C.c_void_p(tower_t.data_ptr()) if tower_t is not None else None,
+            C.c_void_p(logits_t.data_ptr()), C.c_void_p(vlogit_t.data_ptr()), n, int(impl), stream_ptr), "rz_net_debug_heads_impl_dev")
+
+    def select_impl(self, n):
+        """the implementation IMPL_AUTO runs for a batch of n positions"""
+        impl = C.c_int()
+        _cabi.check(_cabi.lib().rz_net_select_impl(self._h, n, C.byref(impl)), "rz_net_select_impl")
+        return impl.value
 
     def close(self):
         if self._h:

@@ -1,0 +1,231 @@
+"""NBoard protocol 2 engine (reference play_game/nboard.py:23-333): ``python -m reversi_zero_b200.run nboard -c <yml>``
+(or the ``nboard_engine`` launcher) lets the NBoard GUI, NTest matches or reversi-arena play and analyse with a model
+of this project.
+
+Commands arrive on stdin, one per line; stdout carries protocol replies only (logging goes to the log file that
+``run.py`` sets up).  ``go`` and ``hint`` search with the one-slot ``ReversiPlayer`` mirror, whose simulations run on
+the device; the tree is kept across the moves of a game and dropped when NBoard sends the opening position.  A
+``ping`` interrupts a running search from the reader thread, so NBoard gets its ``pong`` as soon as the current chunk
+of ``hint_callback_per_sim`` simulations ends.
+"""
+import re
+import sys
+from collections import namedtuple
+from logging import getLogger, StreamHandler, FileHandler
+from time import time
+
+from ..agent.player import ReversiPlayer, CallbackInMCTS
+from ..env.reversi_env import ReversiEnv, Player
+from ..lib.ggf import parse_ggf, convert_to_bitboard_and_actions, convert_move_to_action, convert_action_to_move
+from ..lib.nonblocking_stream_reader import NonBlockingStreamReader
+from .common import load_model
+
+logger = getLogger(__name__)
+
+GameState = namedtuple("GameState", "black white actions player")
+GoResponse = namedtuple("GoResponse", "action eval time")
+HintResponse = namedtuple("HintResponse", "action value visit")
+
+
+def start(config):
+    config.play_with_human.update_play_config(config.play)
+    root_logger = getLogger()
+    for h in list(root_logger.handlers):
+        if isinstance(h, StreamHandler) and not isinstance(h, FileHandler):
+            root_logger.removeHandler(h)
+    logger.info(f"config type={config.type}")
+    NBoardEngine(config).start()
+    logger.info("finish nboard")
+
+
+class NBoardEngine:
+    def __init__(self, config, stdin=None, stdout=None):
+        self.config = config
+        self.stdout = stdout or sys.stdout
+        self.reader = NonBlockingStreamReader(stdin or sys.stdin)
+        self.handler = NBoardProtocolVersion2(config, self)
+        self.running = False
+        self.nc = self.config.nboard
+        self.env = ReversiEnv().reset()
+        self.model = load_model(self.config)
+        self.play_config = self.config.play
+        self.player = self.create_player()
+        self.turn_of_nboard = None
+
+    def create_player(self):
+        logger.debug("create new ReversiPlayer()")
+        return ReversiPlayer(self.config, self.model, self.play_config, enable_resign=False)
+
+    def start(self):
+        """Handles lines until the stream ends.  Lines that arrived before the end are still handled (the reference
+        leaves as soon as its reader sees the end, dropping them)."""
+        self.running = True
+        self.reader.start(push_callback=self.push_callback)
+        while self.running:
+            closed = self.reader.closed   # read before polling: every line is queued before the stream is marked closed
+            message = self.reader.readline(self.nc.read_stdin_timeout)
+            if message is None:
+                if closed:
+                    break
+                continue
+            message = message.strip()
+            logger.debug(f"> {message}")
+            self.handler.handle_message(message)
+
+    def push_callback(self, message):
+        # called on the reader thread: a ping ends the running search
+        if message.startswith("ping"):
+            self.stop_thinking()
+
+    def stop(self):
+        self.running = False
+
+    def reply(self, message):
+        logger.debug(f"< {message}")
+        self.stdout.write(message + "\n")
+        self.stdout.flush()
+
+    def stop_thinking(self):
+        self.player.stop_thinking()
+
+    def set_depth(self, n):
+        """nboard.py:79-91: depth n asks for n * simulation_num_per_depth_about visits on the chosen move, with up to
+        min(30, 5 x that / simulation_num_per_move) thinking loops."""
+        try:
+            n = int(n)
+            self.play_config.required_visit_to_decide_action = n * self.nc.simulation_num_per_depth_about
+            self.play_config.thinking_loop = min(
+                30, int(self.play_config.required_visit_to_decide_action * 5 / self.play_config.simulation_num_per_move))
+            logger.info(f"set required_visit_to_decide_action to {self.play_config.required_visit_to_decide_action}")
+        except ValueError:
+            pass
+
+    def reset_state(self):
+        self.player.engine.close()
+        self.player = self.create_player()
+
+    def set_game(self, game_state):
+        self.env.reset()
+        self.env.update(game_state.black, game_state.white, game_state.player)
+        self.turn_of_nboard = game_state.player
+        for action in game_state.actions:
+            self._change_turn()
+            if action is not None:
+                self.env.step(action)
+
+    def _change_turn(self):
+        if self.turn_of_nboard:
+            self.turn_of_nboard = Player.black if self.turn_of_nboard == Player.white else Player.white
+
+    def move(self, action):
+        self._change_turn()
+        if action is not None:
+            self.env.step(action)
+
+    def _states(self):
+        board = self.env.board
+        return (board.black, board.white) if self.env.next_player == Player.black else (board.white, board.black)
+
+    def go(self):
+        if self.env.next_player != self.turn_of_nboard:   # NBoard's side to move has no legal move: pass
+            return GoResponse(None, 0, 0)
+        states = self._states()
+        start_time = time()
+        action = self.player.action(*states)
+        item = self.player.ask_thought_about(*states)
+        return GoResponse(action, item.values[action], time() - start_time)
+
+    def hint(self, n_hint):
+        states = self._states()
+
+        def hint_report_callback(values, visits):
+            hint_list = []
+            for action, visit in list(sorted(enumerate(visits), key=lambda x: -x[1]))[:n_hint]:
+                if visit > 0:
+                    hint_list.append(HintResponse(action, values[action], visit))
+            self.handler.report_hint(hint_list)
+
+        self.player.action(*states, callback_in_mtcs=CallbackInMCTS(self.nc.hint_callback_per_sim, hint_report_callback))
+        item = self.player.ask_thought_about(*states)
+        hint_report_callback(item.values, item.visit)
+
+
+class NBoardProtocolVersion2:
+    """nboard.py:154-333; the protocol is described at https://github.com/weltyc/ntest/blob/master/instructions/Protocol.htm"""
+
+    def __init__(self, config, engine):
+        self.config = config
+        self.engine = engine
+        self.handlers = [
+            (re.compile(r'nboard ([0-9]+)'), self.nboard),
+            (re.compile(r'set depth ([0-9]+)'), self.set_depth),
+            (re.compile(r'set game (.+)'), self.set_game),
+            (re.compile(r'move ([^/]+)(/[^/]*)?(/[^/]*)?'), self.move),
+            (re.compile(r'hint ([0-9]+)'), self.hint),
+            (re.compile(r'go'), self.go),
+            (re.compile(r'ping ([0-9]+)'), self.ping),
+            (re.compile(r'learn'), self.learn),
+            (re.compile(r'analyze'), self.analyze),
+        ]
+
+    def handle_message(self, message):
+        for regexp, func in self.handlers:
+            match = regexp.match(message)
+            if match:
+                func(*match.groups())
+                return
+        logger.debug(f"ignore message: {message}")
+
+    def nboard(self, version):
+        if version != "2":
+            logger.warning(f"UNKNOWN NBoard Version {version}!!!")
+        self.engine.reply(f"set myname {self.config.nboard.my_name}({self.config.type})")
+        self.tell_status("waiting")
+
+    def set_depth(self, depth):
+        self.engine.set_depth(depth)
+
+    def set_game(self, ggf_str):
+        """The position at the end of the GGF game ``ggf_str``; a game of at most one move starts a new game, which
+        drops the search tree."""
+        ggf = parse_ggf(ggf_str)
+        black, white, actions = convert_to_bitboard_and_actions(ggf)
+        player = Player.black if ggf.BO.color == "*" else Player.white
+        self.engine.set_game(GameState(black, white, actions, player))
+        if len(actions) <= 1:
+            self.engine.reset_state()
+
+    def move(self, move, evaluation, time_sec):
+        self.engine.move(convert_move_to_action(move))
+
+    def hint(self, n):
+        self.tell_status("thinkng hint...")
+        self.engine.hint(int(n))
+        self.tell_status("waiting")
+
+    def report_hint(self, hint_list):
+        for hint in reversed(hint_list):  # NBoard takes the last line as the best
+            move = convert_action_to_move(hint.action)
+            self.engine.reply(f"search {move} {hint.value} 0 {int(hint.visit)}")
+
+    def go(self):
+        """Replies "=== {move}/{eval}/{time}"; the engine's board is not changed (NBoard sends a "move" next)."""
+        self.tell_status("thinking...")
+        gr = self.engine.go()
+        move = convert_action_to_move(gr.action)
+        self.engine.reply(f"=== {move}/{gr.eval * 10}/{gr.time}")
+        self.tell_status("waiting")
+
+    def ping(self, n):
+        # the search has already been stopped by NBoardEngine.push_callback on the reader thread
+        self.engine.reply(f"pong {n}")
+
+    def learn(self):
+        self.engine.reply("learned")
+
+    def analyze(self):
+        """Retrograde analysis is optional in the protocol; the reference leaves it out as well."""
+        pass
+
+    def tell_status(self, status):
+        self.engine.reply(f"status {status}")
