@@ -67,6 +67,33 @@ constexpr uint32_t kSmemAlloc = kSmemBytes + 128;  // slack for manual 128 B ali
 static_assert(kSmemAlloc <= 232448, "shared memory budget exceeded");
 static_assert(kTowerResFloatsPerCta == (size_t)kMathThreads * 128, "residual scratch per CTA");
 
+// Phase stamps (build with -DRZ_TOWER_STAMPS; tools/tower_phases.py): SM-clock deltas summed per CTA into
+// g_tower_stamps[blockIdx.x][phase], as seen by math thread 0 (warpgroup 0) and, for kStEmpty, by the producer thread.
+// Off by default: RZ_STAMP(...) expands to nothing and the production kernel is compiled as if the stamps did not exist.
+#ifdef RZ_TOWER_STAMPS
+enum : int {
+    kStTiles,    // tiles processed (a count, not cycles)
+    kStTile,     // whole tile, layer-0 operand to the end of the heads
+    kStKLoop,    // MMA sections of all layers: from the first weight wait to the last wgmma_wait
+    kStFull,     // waiting on bar_full (weights late; the wgmmas already queued keep running meanwhile)
+    kStMma,      // waiting in wgmma_wait (MMA-bound)
+    kStEpiBar,   // waiting at epi_bar around the layer boundaries
+    kStEpi0,     // layer-0 epilogue
+    kStEpi1,     // conv1 epilogues (first conv of a block)
+    kStEpi2,     // conv2 epilogues (second conv of a block), except the last layer's
+    kStEpiLast,  // last layer's epilogue (head 1x1 sums)
+    kStHeads,    // heads
+    kStEmpty,    // producer: waiting on bar_empty (slot not yet released by both CTAs' math warps)
+    kStCount
+};
+constexpr int kStMaxCtas = 1024;
+__device__ unsigned long long g_tower_stamps[kStMaxCtas][kStCount];
+__device__ __forceinline__ void stamp_add(int phase, uint32_t cycles) { atomicAdd(&g_tower_stamps[blockIdx.x][phase], (unsigned long long)cycles); }
+#define RZ_STAMP(...) __VA_ARGS__
+#else
+#define RZ_STAMP(...)
+#endif
+
 // CL = thread-block-cluster size (1 or 2).  With CL = 2 the two CTAs of a cluster each fetch half of every weight
 // stage from L2 and multicast it into both CTAs' shared memory; MMAs and the epilogue stay per-CTA.  A stage may be
 // refilled only after BOTH CTAs' math warps have read it, so the `empty` barriers count the arrivals of 8 warps per CTA.
@@ -116,8 +143,11 @@ __global__ void __launch_bounds__(kThreads, 1) net_tower_kernel(const Params pp)
             for (uint32_t it = 0; it < iters; ++it) {
                 for (int l = 1; l < L; ++l) {
                     const uint8_t* src = reinterpret_cast<const uint8_t*>(p.w) + (size_t)(l - 1) * 36 * kStageBytes;
+                    RZ_STAMP(uint32_t st_empty = 0;)
                     for (int s = 0; s < 36; ++s) {
+                        RZ_STAMP(const uint32_t c0 = (uint32_t)clock();)
                         mbar_wait(bar_empty(stage), phase ^ 1);
+                        RZ_STAMP(st_empty += (uint32_t)clock() - c0;)
                         mbar_expect_tx(bar_full(stage), kStageBytes);
                         if (CL == 1) {
                             bulk_g2s(base + kOffW + stage * kStageBytes, src + (size_t)s * kStageBytes, kStageBytes, bar_full(stage));
@@ -128,6 +158,7 @@ __global__ void __launch_bounds__(kThreads, 1) net_tower_kernel(const Params pp)
                         }
                         if (++stage == kStages) { stage = 0; phase ^= 1; }
                     }
+                    RZ_STAMP(stamp_add(kStEmpty, st_empty);)
                 }
             }
         }
@@ -161,6 +192,7 @@ __global__ void __launch_bounds__(kThreads, 1) net_tower_kernel(const Params pp)
         for (uint32_t it = 0; it < iters; ++it) {
             const uint32_t tile = blockIdx.x + it * gridDim.x;  // may be >= ntiles: dummy tile (no valid board)
             const uint32_t pos0 = tile * 2;
+            RZ_STAMP(const uint32_t st_tile0 = (uint32_t)clock();)
             {   // ---- layer-0 operand: im2col of the two bit planes, K index = tap*2 + plane, padded to 32 ----
                 const int m = et & 127, g = m >> 3, brd = g & 1;
                 const bool valid = pos0 + brd < p.n;
@@ -168,7 +200,8 @@ __global__ void __launch_bounds__(kThreads, 1) net_tower_kernel(const Params pp)
                                      g >> 1);
                 fence_proxy_async();
             }
-            float hs[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};   // head partial sums: (policy 0, policy 1, value) x (board 0, 1)
+            float hs[6];   // head partial sums (policy 0, policy 1, value) x (board 0, 1): set by the last epilogue only, so that
+                           // they do not hold registers through the K loops
             for (int l = 0; l < L; ++l) {
                 // folded BN parameters, double-buffered across layers: this layer's were copied in during the previous
                 // layer; the next layer's (after the last layer: the first layer's, for the next tile) are copied into
@@ -176,31 +209,40 @@ __global__ void __launch_bounds__(kThreads, 1) net_tower_kernel(const Params pp)
                 const float* sc = ss_s + ss_buf * 512;
                 const bool is_conv2 = l > 0 && (l & 1) == 0;   // second conv of a block: add the skip connection
                 float4 rb[kResAhead];   // residual loads in flight (conv2 layers)
+                RZ_STAMP(uint32_t st_c = (uint32_t)clock(), st_bar = 0, st_full = 0, st_mma = 0;)
                 epi_bar();   // operand (written by both warpgroups, made visible to the async proxy) and BN params ready;
                              // every thread is done with layer l - 1's epilogue, so the other BN buffer is free
+                RZ_STAMP(st_bar += (uint32_t)clock() - st_c;)
                 {
                     const size_t nl = l + 1 < L ? (size_t)l + 1 : 0;
                     const uint32_t dst = smem_u32(ss_s + (ss_buf ^ 1) * 512 + et);
                     cp_async_4(dst, p.ss + nl * 512 + et);
                     cp_async_4(dst + 1024, p.ss + nl * 512 + 256 + et);
                 }
+                RZ_STAMP(const uint32_t st_k0 = (uint32_t)clock();)
                 acc_fence(d);
                 if (l == 0) {
+                    RZ_STAMP(st_c = (uint32_t)clock();)
                     mbar_wait(bar_w0, 0);
+                    RZ_STAMP(st_full += (uint32_t)clock() - st_c;)
                     wgmma_fence();
 #pragma unroll
                     for (uint32_t j = 0; j < 2; ++j)
                         wgmma_m64n256k16(d, smem_desc(base + kOffA0 + j * 2 * 2048 + wg * 1024, 2048, 128),
                                          smem_desc(base + kOffW0 + j * 2 * 4096, 4096, 128), j);
                     wgmma_commit();
+                    RZ_STAMP(st_c = (uint32_t)clock();)
                     wgmma_wait<0>();
+                    RZ_STAMP(st_mma += (uint32_t)clock() - st_c;)
                 } else {
                     int prev = -1;
                     for (uint32_t tap = 0; tap < 9; ++tap) {
                         // tap (kh, kw) reads input pixel (y + kh - 1, x + kw - 1): slot offset 2*kh, chunk offset kw
                         const uint32_t a_tap = a_wg + (2 * (tap / 3)) * kActSlot + (tap % 3) * 16;
                         for (uint32_t kb = 0; kb < 4; ++kb) {
+                            RZ_STAMP(st_c = (uint32_t)clock();)
                             mbar_wait(bar_full(stage), phase);
+                            RZ_STAMP(st_full += (uint32_t)clock() - st_c;)
                             const uint32_t b_st = base + kOffW + stage * kStageBytes;
                             wgmma_fence();
 #pragma unroll
@@ -208,7 +250,9 @@ __global__ void __launch_bounds__(kThreads, 1) net_tower_kernel(const Params pp)
                                 wgmma_m64n256k16(d, smem_desc(a_tap + (kb * 8 + 2 * j) * kActCg, kActCg, kActSlot),
                                                  smem_desc(b_st + 2 * j * 4096, 4096, 128), (tap | kb | j) != 0);
                             wgmma_commit();
+                            RZ_STAMP(st_c = (uint32_t)clock();)
                             wgmma_wait<1>();   // the previous stage's MMAs have completed: its slot may be refilled
+                            RZ_STAMP(st_mma += (uint32_t)clock() - st_c;)
                             if (prev >= 0 && lane == 0) {
                                 mbar_arrive(bar_empty(prev));
                                 if (CL > 1) mbar_arrive_cta(bar_empty(prev), crank ^ 1u);
@@ -222,28 +266,42 @@ __global__ void __launch_bounds__(kThreads, 1) net_tower_kernel(const Params pp)
 #pragma unroll
                         for (int i = 0; i < kResAhead; ++i) rb[i] = res[i * 256];
                     }
+                    RZ_STAMP(st_c = (uint32_t)clock();)
                     wgmma_wait<0>();
+                    RZ_STAMP(st_mma += (uint32_t)clock() - st_c;)
                     if (lane == 0) {
                         mbar_arrive(bar_empty(prev));
                         if (CL > 1) mbar_arrive_cta(bar_empty(prev), crank ^ 1u);
                     }
                 }
+                RZ_STAMP(const uint32_t st_k1 = (uint32_t)clock();)
                 acc_fence(d);
                 cp_async_wait_all();   // the next layer's BN parameters have landed (published by the next barrier)
                 ss_buf ^= 1;
                 const bool keep_res = l == 0 || is_conv2;      // block output: keep an fp32 copy for the skip connection
                 const bool last = l == L - 1;
+                RZ_STAMP(st_c = (uint32_t)clock();)
                 if (!last) epi_bar();   // both warpgroups' MMAs have finished reading the operand it is about to overwrite
+                RZ_STAMP(const uint32_t st_e0 = (uint32_t)clock(); st_bar += st_e0 - st_c;)
                 float* dbg0 = nullptr;
                 float* dbg1 = nullptr;
                 if (last && p.dbg_tower) {
                     if (pos0 < p.n) dbg0 = p.dbg_tower + ((size_t)pos0 * 64 + y * 8 + x) * 256;
                     if (pos0 + 1 < p.n) dbg1 = p.dbg_tower + ((size_t)(pos0 + 1) * 64 + y * 8 + x) * 256;
                 }
-                // the epilogue is compiled once with and once without the skip connection, so that a conv2 layer's
-                // residual loads land straight in the registers that consume them kResAhead steps later
-                auto epilogue = [&](auto conv2) {
+                // the epilogue is compiled once per layer kind, so that its unrolled loop holds no branch: the compiler
+                // can then hoist the BN loads and interleave the steps, and a conv2 layer's residual loads land straight
+                // in the registers that consume them kResAhead steps later.  kConv2: add the skip connection; kKind:
+                // kEpiRelu (first conv of a block: ReLU folded into the fp16 convert), kEpiKeep (block output: ReLU, fp32
+                // copy kept for the skip connection), kEpiLast (tower output: ReLU, head 1x1 sums)
+                constexpr int kEpiRelu = 0, kEpiKeep = 1, kEpiLast = 2;
+                auto epilogue = [&](auto conv2, auto kind) {
                     constexpr bool kConv2 = decltype(conv2)::value;
+                    constexpr bool kKeep = decltype(kind)::value == kEpiKeep, kLast = decltype(kind)::value == kEpiLast;
+                    if (kLast) {
+#pragma unroll
+                        for (int k = 0; k < 6; ++k) hs[k] = 0.f;
+                    }
 #pragma unroll
                 for (int i = 0; i < 32; ++i) {
                     const int c = 8 * i + cq;
@@ -256,14 +314,13 @@ __global__ void __launch_bounds__(kThreads, 1) net_tower_kernel(const Params pp)
                         if (i + kResAhead < 32) rb[i % kResAhead] = res[(i + kResAhead) * 256];
                         v0 += r.x; v1 += r.y; v2 += r.z; v3 += r.w;
                     }
-                    if (keep_res || last) {
+                    if (kKeep || kLast) {
                         v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); v2 = fmaxf(v2, 0.f); v3 = fmaxf(v3, 0.f);
                     }
-                    if (!last) {
-                        if (keep_res) res[i * 256] = make_float4(v0, v1, v2, v3);
-                        // the first convolution of a block folds its ReLU into the fp16 convert
-                        const uint32_t h0 = keep_res ? pack_h2<false>(v0, v1) : pack_h2<true>(v0, v1);
-                        const uint32_t h1 = keep_res ? pack_h2<false>(v2, v3) : pack_h2<true>(v2, v3);
+                    if (!kLast) {
+                        if (kKeep) res[i * 256] = make_float4(v0, v1, v2, v3);
+                        const uint32_t h0 = pack_h2<!kKeep>(v0, v1);
+                        const uint32_t h1 = pack_h2<!kKeep>(v2, v3);
                         const uint32_t off = (c >> 3) * kActCg;
                         asm volatile("st.shared.b32 [%0], %1;" ::"r"(act_row0 + off), "r"(h0) : "memory");
                         asm volatile("st.shared.b32 [%0], %1;" ::"r"(act_row1 + off), "r"(h1) : "memory");
@@ -281,10 +338,25 @@ __global__ void __launch_bounds__(kThreads, 1) net_tower_kernel(const Params pp)
                     }
                 }
                 };
-                if (is_conv2) epilogue(std::true_type());
-                else epilogue(std::false_type());
+                using Conv2 = std::true_type;
+                using NoConv2 = std::false_type;
+                if (last) {
+                    if (is_conv2) epilogue(Conv2(), std::integral_constant<int, kEpiLast>());
+                    else epilogue(NoConv2(), std::integral_constant<int, kEpiLast>());   // no residual block: layer 0 is last
+                } else if (is_conv2) {
+                    epilogue(Conv2(), std::integral_constant<int, kEpiKeep>());
+                } else if (keep_res) {
+                    epilogue(NoConv2(), std::integral_constant<int, kEpiKeep>());     // layer 0
+                } else {
+                    epilogue(NoConv2(), std::integral_constant<int, kEpiRelu>());
+                }
                 if (!last) fence_proxy_async();
+                RZ_STAMP(if (et == 0) {
+                    stamp_add(kStKLoop, st_k1 - st_k0); stamp_add(kStFull, st_full); stamp_add(kStMma, st_mma); stamp_add(kStEpiBar, st_bar);
+                    stamp_add(l == 0 ? kStEpi0 : last ? kStEpiLast : is_conv2 ? kStEpi2 : kStEpi1, (uint32_t)clock() - st_e0);
+                })
             }
+            RZ_STAMP(const uint32_t st_h0 = (uint32_t)clock();)
             // ---- heads (agent/model.py:43-56) on the 256 math threads ----------------------------------
             // the four lanes of a row quad hold disjoint column sets of the same two rows
 #pragma unroll
@@ -295,8 +367,14 @@ __global__ void __launch_bounds__(kThreads, 1) net_tower_kernel(const Params pp)
             // lane quad (0, 1, 2, 3) -> (row r0 colhalf 0, row r0 + 8 colhalf 0, r0 colhalf 1 = 0, r0 + 8 colhalf 1 = 0)
             const int q = lane & 3, brd = q & 1, m = r0 + 8 * brd;
             const bool full = q < 2;
-            heads_phase(p, full ? hs[3 * brd] : 0.f, full ? hs[3 * brd + 1] : 0.f, full ? hs[3 * brd + 2] : 0.f, q >> 1, m, brd, y, x, et,
+            // constant indices keep hs in registers (a lane-dependent index would put it in local memory)
+            const float h0 = brd ? hs[3] : hs[0], h1 = brd ? hs[4] : hs[1], h2 = brd ? hs[5] : hs[2];
+            heads_phase(p, full ? h0 : 0.f, full ? h1 : 0.f, full ? h2 : 0.f, q >> 1, m, brd, y, x, et,
                         warp, lane, pos0, part, hp, hv, logit, fc1);
+            RZ_STAMP(if (et == 0) {
+                const uint32_t st_h1 = (uint32_t)clock();
+                stamp_add(kStHeads, st_h1 - st_h0); stamp_add(kStTile, st_h1 - st_tile0); stamp_add(kStTiles, 1);
+            })
         }
     }
 
@@ -397,3 +475,23 @@ int net_forward_tc(rz_net* net, const uint64_t* own, const uint64_t* enemy, floa
 }
 
 }  // namespace rz
+
+#ifdef RZ_TOWER_STAMPS
+// Stamped builds only (tools/tower_phases.py): copies the per-CTA phase sums, [n_ctas][kStCount] uint64, to `out`
+// (when not null), then zeroes them if `reset`.  Returns a cudaError_t.
+extern "C" int rz_tower_stamps(unsigned long long* out, int n_ctas, int reset) {
+    using namespace rz::tc;
+    if (n_ctas < 0 || n_ctas > kStMaxCtas) return (int)cudaErrorInvalidValue;
+    const size_t bytes = (size_t)n_ctas * kStCount * sizeof(unsigned long long);
+    cudaError_t e = cudaDeviceSynchronize();
+    if (e == cudaSuccess && out) e = cudaMemcpyFromSymbol(out, g_tower_stamps, bytes);
+    if (e == cudaSuccess && reset) {
+        void* dev = nullptr;
+        e = cudaGetSymbolAddress(&dev, g_tower_stamps);
+        if (e == cudaSuccess) e = cudaMemset(dev, 0, sizeof(g_tower_stamps));
+        if (e == cudaSuccess) e = cudaDeviceSynchronize();
+    }
+    return (int)e;
+}
+extern "C" int rz_tower_stamp_count() { return rz::tc::kStCount; }
+#endif
