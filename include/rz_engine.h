@@ -110,9 +110,10 @@ typedef struct rz_net_cfg {
     int32_t kernel_size; /* ModelConfig.cnn_filter_size  (config.py:190); only 3 is supported */
 } rz_net_cfg;
 
-#define RZ_NET_IMPL_AUTO 0    /* wgmma tower when filters == 256, else the generic kernel */
-#define RZ_NET_IMPL_GENERIC 1 /* CUDA-core fp32 kernel, any configuration */
-#define RZ_NET_IMPL_TCGEN05 2 /* fused persistent tensor-core (wgmma) tower (filters must be 256) */
+#define RZ_NET_IMPL_AUTO 0    /* wgmma tower when filters is 64, 128 or 256 and value_fc <= 512, else the generic kernel */
+#define RZ_NET_IMPL_GENERIC 1 /* CUDA-core fp32 kernel, any configuration (the exact path) */
+#define RZ_NET_IMPL_TCGEN05 2 /* fused persistent tensor-core (wgmma) tower, fp16 operands / fp32 accumulation (filters must
+                                 be 64, 128 or 256, value_fc <= 512) */
 #define RZ_NET_IMPL_SPLIT 3   /* the same tower with each 2-board tile split over an 8-CTA cluster: lower latency for small
                                  batches, bit-identical outputs (filters must be 256); AUTO picks it up to a measured batch size */
 
@@ -138,7 +139,7 @@ int rz_net_load_weights_dev(rz_net* net, const float* blob_dev, size_t n_floats,
 int rz_net_predict_dev(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value,
                        size_t n, int impl, void* stream);
 /* diagnostic variant of the tensor-core tower path: additionally writes the fp32 residual-tower output
- * tower[n][64 pixels][256 channels] (pixel = y*8+x) so tests can localise a numerical difference. */
+ * tower[n][64 pixels][filters channels] (pixel = y*8+x) so tests can localise a numerical difference. */
 int rz_net_debug_tower_dev(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value,
                            float* tower, size_t n, void* stream);
 /* same, plus the head outputs BEFORE softmax / tanh -- policy_logits[n][64] (the input of the policy_out softmax,

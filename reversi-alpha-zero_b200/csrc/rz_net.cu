@@ -7,6 +7,7 @@
 #include <new>
 #include "rz_bitboard.cuh"
 #include "rz_net.cuh"
+#include "rz_tc_common.cuh"
 
 namespace rz {
 
@@ -181,9 +182,13 @@ int net_forward_generic(rz_net* net, const uint64_t* own, const uint64_t* enemy,
 // 0.99 vs 0.50 ms), tools/search_latency_bench.py, DESIGN.md §5 "Split tower".
 constexpr size_t kSplitMaxBatch = 0;
 
+// AUTO: the wgmma tower for every width it has (64, 128, 256 filters) and value heads it holds; the generic fp32 kernel
+// for everything else.  The narrow tower was faster than the generic kernel at every batch size measured (DESIGN.md §6
+// "Narrow towers"), so it has no batch threshold.
 int select_impl(const rz_net* net, size_t n, int impl) {
     if (impl != RZ_NET_IMPL_AUTO) return impl;
-    if (net->cfg.filters != 256) return RZ_NET_IMPL_GENERIC;
+    if (!tc_width(net->cfg.filters) || net->cfg.value_fc > (int)tc::kTcMaxV) return RZ_NET_IMPL_GENERIC;
+    if (net->cfg.filters != 256) return RZ_NET_IMPL_TCGEN05;
     return n <= kSplitMaxBatch ? RZ_NET_IMPL_SPLIT : RZ_NET_IMPL_TCGEN05;
 }
 
@@ -193,9 +198,12 @@ int net_forward(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* 
     if (n == 0) return RZ_OK;
     impl = select_impl(net, n, impl);
     if (impl == RZ_NET_IMPL_TCGEN05 || impl == RZ_NET_IMPL_SPLIT) {
-        RZ_REQUIRE(net->cfg.filters == 256, "tensor-core towers require filters == 256 (got %d)", net->cfg.filters);
-        return impl == RZ_NET_IMPL_SPLIT ? net_forward_split(net, own, enemy, policy, value, n, stream, nullptr)
-                                         : net_forward_tc(net, own, enemy, policy, value, n, stream, nullptr);
+        if (impl == RZ_NET_IMPL_SPLIT) {
+            RZ_REQUIRE(net->cfg.filters == 256, "the split tower requires filters == 256 (got %d)", net->cfg.filters);
+            return net_forward_split(net, own, enemy, policy, value, n, stream, nullptr);
+        }
+        RZ_REQUIRE(tc_width(net->cfg.filters), "the tensor-core tower requires filters 64, 128 or 256 (got %d)", net->cfg.filters);
+        return net_forward_tc(net, own, enemy, policy, value, n, stream, nullptr);
     }
     RZ_REQUIRE(impl == RZ_NET_IMPL_GENERIC, "unknown net impl %d", impl);
     return net_forward_generic(net, own, enemy, policy, value, n, stream);
@@ -224,6 +232,7 @@ static int finish_load(rz_net* net, cudaStream_t stream) {
     fold_bn_kernel<<<1, 32, 0, stream>>>(net->blob, net->off_value_conv, (size_t)F, 1, ssh + 4, ssh + 5);
     RZ_LAUNCH_CHECK();
     if (F == 256) RZ_TRY(net_pack_tc(net, stream));
+    else if (tc_width(F)) RZ_TRY(net_pack_tc_narrow(net, stream));
     RZ_CUDA_TRY(cudaStreamSynchronize(stream));
     net->loaded = true;
     return RZ_OK;
@@ -262,9 +271,9 @@ int rz_net_create(const rz_net_cfg* cfg, int device, rz_net** out) {
     net->blob_floats = off;
     cudaError_t e = cudaMalloc(&net->blob, off * sizeof(float));
     if (e == cudaSuccess) e = cudaMalloc(&net->scale_shift, ss_floats(*cfg) * sizeof(float));
-    if (e == cudaSuccess && F == 256) {
-        e = cudaMalloc(&net->tc_w0, (size_t)4 * 256 * 8 * sizeof(__half));
-        if (e == cudaSuccess && R > 0) e = cudaMalloc(&net->tc_w, (size_t)2 * R * 36 * 8 * 256 * 8 * sizeof(__half));
+    if (e == cudaSuccess && tc_width((int)F)) {   // packed fp16 images (9 F^2 halves per conv), residual scratch
+        e = cudaMalloc(&net->tc_w0, (size_t)4 * F * 8 * sizeof(__half));
+        if (e == cudaSuccess && R > 0) e = cudaMalloc(&net->tc_w, (size_t)2 * R * 9 * F * F * sizeof(__half));
         if (e == cudaSuccess) e = cudaMalloc(&net->res, (size_t)num_sms() * kTowerResFloatsPerCta * sizeof(float));
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&net->res_done, cudaEventDisableTiming);
     }
@@ -336,7 +345,7 @@ int rz_net_debug_heads_impl_dev(rz_net* net, const uint64_t* own, const uint64_t
                                 float* policy_logits, float* value_logit, size_t n, int impl, void* stream) {
     RZ_REQUIRE(net && own && enemy && policy && value && policy_logits && value_logit, "rz_net_debug_heads_impl_dev: null pointer");
     if (!net->loaded) { set_error("rz_net: weights not loaded"); return RZ_ESTATE; }
-    RZ_REQUIRE(net->cfg.filters == 256, "tensor-core towers require filters == 256 (got %d)", net->cfg.filters);
+    RZ_REQUIRE(tc_width(net->cfg.filters), "the tensor-core tower requires filters 64, 128 or 256 (got %d)", net->cfg.filters);
     if (n == 0) return RZ_OK;
     impl = select_impl(net, n, impl);
     if (impl == RZ_NET_IMPL_SPLIT)

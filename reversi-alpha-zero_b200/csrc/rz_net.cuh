@@ -21,9 +21,10 @@ struct rz_net {
     size_t off_conv0, off_res0, res_stride_conv;  // kernel offset of conv0; of res0.conv1; floats per (conv+bn) group
     size_t off_policy_conv, off_policy_fc_k, off_policy_fc_b;
     size_t off_value_conv, off_value_fc1_k, off_value_fc1_b, off_value_fc2_k, off_value_fc2_b;
-    // wgmma tower (F == 256 only)
-    __half* tc_w0;       // [4 kc][256 n][8] fp16: layer-0 weights, K = 18 padded to 32, K-major no-swizzle image
-    __half* tc_w;        // [2R layers][36 stages][8 kc][256 n][8] fp16: one 32 KB shared-memory image per pipeline stage
+    // wgmma tower (F == 64, 128 or 256)
+    __half* tc_w0;       // [4 kc][F n][8] fp16: layer-0 weights, K = 18 padded to 32, K-major no-swizzle image
+    __half* tc_w;        // F = 256: [2R layers][36 stages][8 kc][256 n][8] fp16, one 32 KB shared-memory image per pipeline stage;
+                         // F = 64 / 128: [2R layers][9 taps][F/8 kc][F n][8] fp16, a stage is 3 / 1 consecutive taps
     // fp32 residual-stream scratch of the tower kernel ([CTA][kTowerResFloatsPerCta]); launches from different streams
     // are ordered through res_done, recorded after every launch that uses it
     float* res;
@@ -46,8 +47,9 @@ int net_forward_generic(rz_net* net, const uint64_t* own, const uint64_t* enemy,
 // batch size known only on the device (count_dev), at most max_n
 int net_forward_counted(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value,
                         const uint32_t* count_dev, size_t max_n, int impl, cudaStream_t stream);
+// the wgmma tower for F = 256 (rz_net_tc.cu) and, through net_forward_tc_narrow, F = 64 and 128
 int net_forward_tc(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value, size_t n,
-                   cudaStream_t stream, float* dbg_tower /* nullable: [n][64][256] fp32 tower output */,
+                   cudaStream_t stream, float* dbg_tower /* nullable: [n][64][F] fp32 tower output */,
                    const uint32_t* n_dev = nullptr /* nullable: actual batch size in device memory (<= n) */,
                    float* dbg_logits = nullptr /* nullable: [n][64] policy logits */, float* dbg_vlogit = nullptr /* nullable: [n] */);
 // same function as net_forward_tc, bit for bit, one 8-CTA cluster per 2-board tile (small batches, rz_net_split.cu)
@@ -57,8 +59,14 @@ int net_forward_split(rz_net* net, const uint64_t* own, const uint64_t* enemy, f
 // RZ_NET_IMPL_AUTO -> the implementation used for a batch of capacity n
 int select_impl(const rz_net* net, size_t n, int impl);
 int net_pack_tc(rz_net* net, cudaStream_t stream);
-// thread-block clusters of the tower kernel: 2 = CTA pairs sharing the weight stages (default), 1 = single CTAs
+// the same tower for 64 and 128 filters, B = 512 / F boards per tile (rz_net_tc_narrow.cu)
+int net_forward_tc_narrow(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value, size_t n,
+                          cudaStream_t stream, float* dbg_tower, const uint32_t* n_dev, float* dbg_logits, float* dbg_vlogit);
+int net_pack_tc_narrow(rz_net* net, cudaStream_t stream);
+inline bool tc_width(int filters) { return filters == 64 || filters == 128 || filters == 256; }
+// thread-block clusters of the tower kernels: 2 = CTA pairs sharing the weight stages (default), 1 = single CTAs
 int set_tower_cluster(int cluster);
+int tower_cluster();   // the current setting: rz_net_set_tower_cluster, else RZ_TOWER_CLUSTER, else 2
 int net_forward(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value, size_t n, int impl,
                 cudaStream_t stream);
 

@@ -420,9 +420,19 @@ int set_tower_cluster(int cluster) {
     return RZ_OK;
 }
 
+int tower_cluster() {
+    if (g_cluster == 0) {
+        const char* cs = getenv("RZ_TOWER_CLUSTER");
+        g_cluster = (cs && atoi(cs) == 1) ? 1 : 2;
+    }
+    return g_cluster;
+}
+
 int net_forward_tc(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value, size_t n, cudaStream_t stream,
                    float* dbg_tower, const uint32_t* n_dev, float* dbg_logits, float* dbg_vlogit) {
-    RZ_REQUIRE(net->cfg.filters == 256, "wgmma tower requires 256 filters");
+    if (net->cfg.filters == 64 || net->cfg.filters == 128)
+        return net_forward_tc_narrow(net, own, enemy, policy, value, n, stream, dbg_tower, n_dev, dbg_logits, dbg_vlogit);
+    RZ_REQUIRE(net->cfg.filters == 256, "wgmma tower requires 64, 128 or 256 filters (got %d)", net->cfg.filters);
     RZ_REQUIRE(net->cfg.value_fc <= (int)tc::kTcMaxV, "wgmma tower supports value_fc_size <= %u", tc::kTcMaxV);
     RZ_REQUIRE(n < (1ull << 31), "batch too large");
     static int max_pairs = -1;
@@ -438,11 +448,7 @@ int net_forward_tc(rz_net* net, const uint64_t* own, const uint64_t* enemy, floa
         cfg.attrs = attr; cfg.numAttrs = 1;
         RZ_CUDA_TRY(cudaOccupancyMaxActiveClusters(&max_pairs, tc::net_tower_kernel<2>, &cfg));
     }
-    if (g_cluster == 0) {
-        const char* cs = getenv("RZ_TOWER_CLUSTER");
-        g_cluster = (cs && atoi(cs) == 1) ? 1 : 2;
-    }
-    const int cluster = g_cluster == 2 && max_pairs >= 1 ? 2 : 1;
+    const int cluster = tower_cluster() == 2 && max_pairs >= 1 ? 2 : 1;
     tc::Params p;
     p.w0 = net->tc_w0; p.w = net->tc_w; p.ss = net->scale_shift; p.blob = net->blob;
     p.off_policy_conv = net->off_policy_conv; p.off_policy_fc_k = net->off_policy_fc_k; p.off_policy_fc_b = net->off_policy_fc_b;

@@ -1,0 +1,498 @@
+// rz_net_tc_narrow.cu -- the fused persistent wgmma tower of rz_net_tc.cu for the 64- and 128-filter networks (sm_90a).
+//
+// Same machine as net_tower_kernel (rz_net_tc.cu; DESIGN.md §5), with the tile widened so that every MMA keeps the
+// 128-row x 256-column accumulator footprint of the 256-filter kernel:
+//   * a tile holds B = 512 / F boards (4 at 128 filters, 8 at 64): M = 64 B pixel rows, two math warpgroups of 32 B rows;
+//   * each math warpgroup issues T = 256 / F wgmma.m64nFk16 per k-step, one per 64-row sub-tile, all with the same B
+//     (weight) descriptor; sub-tile t accumulates into d[t * F/2 ...] of the thread's 128 fp32 registers;
+//   * activations: fp16, K-major no-swizzle, one-pixel zero border, slot = B*(y+1) + board (a dy shift is B slots):
+//         chunk(cg, slot, xp) at cg*kActCg + slot*144 + xp*16,  kActCg = B*10*144 + 16  (92.4 KB / 92.3 KB)
+//     MMA row m = (B*y + board)*8 + x; rows r and r + 8 of a thread are the same pixel of boards b and b + 1 (b even);
+//   * weights: fp16 stages of TPS taps x F input x F output channels streamed through a 3-deep mbarrier ring by one
+//     producer thread (multicast across a CTA pair with CL = 2): one tap (32 KB, 9 stages per conv) at 128 filters, one
+//     kernel row of three taps (24 KB, 3 stages per conv) at 64 filters;
+//   * epilogue (folded BN, skip connection from the per-CTA fp32 residual scratch, ReLU, fp16 operand for the next layer),
+//     layer 0 (im2col GEMM, K = 18 padded to 32) and heads as in rz_net_tc.cu, for B boards.  A row's 1x1 head-conv sums
+//     are complete in its lane quad, so the heads need no cross-warpgroup partial-sum array.
+// Every output element goes through the same operations whichever tile slot its board lands in.
+#include <stdlib.h>
+#include <mutex>
+#include <type_traits>
+#include "rz_bitboard.cuh"
+#include "rz_net.cuh"
+#include "rz_tc_common.cuh"
+
+namespace rz {
+namespace tc {
+namespace narrow {
+
+constexpr int kThreads = 384;
+constexpr uint32_t kProducerRegs = 40, kMathRegs = 232;
+constexpr uint32_t kActSlot = 144;
+constexpr uint32_t kStages = 3;
+constexpr int kResAhead = 4;
+
+template <int F>
+struct Cfg {
+    static_assert(F == 64 || F == 128, "narrow tower: 64 or 128 filters");
+    static constexpr int B = 512 / F;                 // boards per tile
+    static constexpr int T = 256 / F;                 // 64-row sub-tiles (MMAs per k-step) per math warpgroup
+    static constexpr int TPS = F == 128 ? 1 : 3;      // taps per weight stage
+    static constexpr int S = 9 / TPS;                 // weight stages per conv layer
+    static constexpr int KPT = F / 16;                // k16 steps per tap
+    static constexpr uint32_t kActCg = B * 10 * kActSlot + 16;
+    static constexpr uint32_t kActBytes = (F / 8) * kActCg;
+    static constexpr uint32_t kTapBytes = F * F * 2;  // one tap's [F/8 kc][F n][8] fp16 image
+    static constexpr uint32_t kStageBytes = TPS * kTapBytes;
+    static constexpr uint32_t kA0Kc = B * 8 * 128;    // layer-0 operand: bytes per 8-wide K chunk (8B board rows x 8 x 16 B)
+    static constexpr uint32_t kA0Bytes = 4 * kA0Kc;
+    static constexpr uint32_t kW0Bytes = 4 * F * 16;
+    static constexpr uint32_t kOffAct = 0;
+    static constexpr uint32_t kOffW = kOffAct + kActBytes;
+    static constexpr uint32_t kOffA0 = kOffW + kStages * kStageBytes;
+    static constexpr uint32_t kOffW0 = kOffA0 + kA0Bytes;
+    static constexpr uint32_t kOffSS = kOffW0 + kW0Bytes;           // 2 x [scale F][shift F] fp32
+    static constexpr uint32_t kOffHw = kOffSS + 2 * 2 * F * 4;      // 1x1 head-conv weights: policy [F][2], value [F] fp32
+    static constexpr uint32_t kOffHp = kOffHw + 3 * F * 4;          // [B][128]
+    static constexpr uint32_t kOffHv = kOffHp + B * 128 * 4;        // [B][64]
+    static constexpr uint32_t kOffLogit = kOffHv + B * 64 * 4;      // [B][64]
+    static constexpr uint32_t kOffFc1 = kOffLogit + B * 64 * 4;     // [B][kTcMaxV]
+    static constexpr uint32_t kOffBar = kOffFc1 + B * kTcMaxV * 4;  // full[], empty[], w0
+    static constexpr uint32_t kSmemBytes = kOffBar + (2 * kStages + 1) * 8;
+    static constexpr uint32_t kSmemAlloc = kSmemBytes + 128;        // slack for manual 128 B alignment
+    static_assert(kSmemAlloc <= 232448, "shared memory budget exceeded");
+    static_assert(kActBytes % 16 == 0 && kOffW % 128 == 0 && kStageBytes % (16 * 2) == 0 && kOffA0 % 128 == 0 && kOffW0 % 128 == 0,
+                  "operand and bulk-copy alignment");
+    static_assert(T * F / 2 == 128 && T * (F / 8) == 32, "128 accumulators = 32 residual float4 per thread");
+};
+static_assert(kTowerResFloatsPerCta == (size_t)256 * 128, "residual scratch per CTA");
+
+// the 256 / F MMAs of one k-step of a math warpgroup: sub-tile t reads the A rows at a + t * a_step and accumulates into
+// d[t * F/2 ..]; all of them share the weight descriptor
+template <int F>
+__device__ __forceinline__ void mma_kstep(float (&d)[128], uint32_t a, uint32_t a_step, uint32_t lbo, uint32_t sbo, uint64_t bdesc,
+                                          uint32_t accumulate) {
+    if constexpr (F == 128) {
+        wgmma_m64n128k16<0>(d, smem_desc(a, lbo, sbo), bdesc, accumulate);
+        wgmma_m64n128k16<64>(d, smem_desc(a + a_step, lbo, sbo), bdesc, accumulate);
+    } else {
+        wgmma_m64n64k16<0>(d, smem_desc(a, lbo, sbo), bdesc, accumulate);
+        wgmma_m64n64k16<32>(d, smem_desc(a + a_step, lbo, sbo), bdesc, accumulate);
+        wgmma_m64n64k16<64>(d, smem_desc(a + 2 * a_step, lbo, sbo), bdesc, accumulate);
+        wgmma_m64n64k16<96>(d, smem_desc(a + 3 * a_step, lbo, sbo), bdesc, accumulate);
+    }
+}
+
+// layer-0 im2col of one board row (g, x) for K chunks kc0, kc0 + 1 (build_layer0_operand with a K-chunk stride of kKc)
+template <uint32_t kKc>
+__device__ __forceinline__ void build_layer0_rows(uint8_t* a0, u64 o, u64 e, int kc0, int g, int x, int y) {
+#pragma unroll
+    for (int kk = 0; kk < 2; ++kk) {
+        const int kc = kc0 + kk;
+        uint32_t w[4];
+#pragma unroll
+        for (int jp = 0; jp < 4; ++jp) {
+            uint32_t packed = 0;
+#pragma unroll
+            for (int half = 0; half < 2; ++half) {
+                const int k = kc * 8 + jp * 2 + half;
+                uint32_t bit = 0;
+                if (k < 18) {
+                    const int tap = k >> 1, yy = y + tap / 3 - 1, xx = x + tap % 3 - 1;
+                    if (yy >= 0 && yy < 8 && xx >= 0 && xx < 8) bit = (uint32_t)((((k & 1) ? e : o) >> (yy * 8 + xx)) & 1ULL);
+                }
+                packed |= (bit ? 0x3C00u : 0u) << (16 * half);  // fp16 1.0
+            }
+            w[jp] = packed;
+        }
+        *reinterpret_cast<uint4*>(a0 + kc * kKc + g * 128 + x * 16) = make_uint4(w[0], w[1], w[2], w[3]);
+    }
+}
+
+// CL = thread-block-cluster size (1 or 2), as in net_tower_kernel
+template <int F, int CL>
+__global__ void __launch_bounds__(kThreads, 1) net_tower_narrow_kernel(const Params pp) {
+    using C = Cfg<F>;
+    constexpr int B = C::B, T = C::T;
+    Params p = pp;
+    if (p.n_dev) p.n = *p.n_dev;
+    extern __shared__ uint8_t smem_raw[];
+    const uint32_t base = (smem_u32(smem_raw) + 127u) & ~127u;
+    uint8_t* sm = smem_raw + (base - smem_u32(smem_raw));
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint32_t bar0 = base + C::kOffBar;
+    auto bar_full = [&](uint32_t s) { return bar0 + s * 8; };
+    auto bar_empty = [&](uint32_t s) { return bar0 + (kStages + s) * 8; };
+    const uint32_t bar_w0 = bar0 + 2 * kStages * 8;
+    const uint32_t ntiles = (p.n + B - 1) / B;
+    const int L = p.n_layers;
+    const uint32_t crank = CL > 1 ? cluster_ctarank() : 0u;
+    const uint32_t cbase = blockIdx.x - crank;
+    const uint32_t iters = cbase < ntiles ? (ntiles - cbase + gridDim.x - 1) / gridDim.x : 0u;
+
+    // ---- one-time setup -----------------------------------------------------------------------------
+    for (uint32_t i = threadIdx.x * 16; i < C::kActBytes; i += kThreads * 16) *reinterpret_cast<uint4*>(sm + C::kOffAct + i) = make_uint4(0, 0, 0, 0);
+    fence_proxy_async();
+    for (uint32_t i = threadIdx.x; i < 3 * F; i += kThreads)
+        reinterpret_cast<float*>(sm + C::kOffHw)[i] = __ldg(i < 2 * F ? p.blob + p.off_policy_conv + i : p.blob + p.off_value_conv + (i - 2 * F));
+    if (threadIdx.x == 0) {
+        for (uint32_t s = 0; s < kStages; ++s) { mbar_init(bar_full(s), 1); mbar_init(bar_empty(s), 8 * CL); }
+        mbar_init(bar_w0, 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    if (CL > 1) cluster_sync_all();
+
+    if (warp >= 8) {
+        // ===== weight producer =====================================================================
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProducerRegs));
+        if (warp == 8 && lane == 0) {
+            if (iters > 0) {
+                mbar_expect_tx(bar_w0, C::kW0Bytes);
+                bulk_g2s(base + C::kOffW0, p.w0, C::kW0Bytes, bar_w0);
+            }
+            uint32_t stage = 0, phase = 0;
+            for (uint32_t it = 0; it < iters; ++it) {
+                for (int l = 1; l < L; ++l) {
+                    const uint8_t* src = reinterpret_cast<const uint8_t*>(p.w) + (size_t)(l - 1) * C::S * C::kStageBytes;
+                    for (int s = 0; s < C::S; ++s) {
+                        mbar_wait(bar_empty(stage), phase ^ 1);
+                        mbar_expect_tx(bar_full(stage), C::kStageBytes);
+                        if (CL == 1) {
+                            bulk_g2s(base + C::kOffW + stage * C::kStageBytes, src + (size_t)s * C::kStageBytes, C::kStageBytes, bar_full(stage));
+                        } else {
+                            constexpr uint32_t kSlice = C::kStageBytes / CL;
+                            bulk_g2s_mc(base + C::kOffW + stage * C::kStageBytes + crank * kSlice, src + (size_t)s * C::kStageBytes + crank * kSlice,
+                                        kSlice, bar_full(stage), (uint16_t)((1u << CL) - 1u));
+                        }
+                        if (++stage == kStages) { stage = 0; phase ^= 1; }
+                    }
+                }
+            }
+        }
+    } else {
+        // ===== math warpgroups (2) =================================================================
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kMathRegs));
+        const int et = threadIdx.x;   // 0..255
+        const int wg = warp >> 2;     // MMA rows wg*64T .. wg*64T + 64T - 1
+        const int x = lane >> 2, cq = 2 * (lane & 3);
+        // sub-tile t: board rows g_t = g0 + 8t (board g_t % B at y = g_t / B) and g_t + 1 (the next board), pixel column x
+        const int g0 = wg * T * 8 + (warp & 3) * 2;
+        const uint32_t act_row0 = base + C::kOffAct + (g0 + B) * kActSlot + (x + 1) * 16 + cq * 2;  // + 8t*kActSlot + cg*kActCg
+        const uint32_t a_wg = base + C::kOffAct + wg * T * 8 * kActSlot;                            // + 8t*kActSlot: sub-tile t
+        float* ss_s = reinterpret_cast<float*>(sm + C::kOffSS);
+        float* hp = reinterpret_cast<float*>(sm + C::kOffHp);
+        float* hv = reinterpret_cast<float*>(sm + C::kOffHv);
+        float* logit = reinterpret_cast<float*>(sm + C::kOffLogit);
+        float* fc1 = reinterpret_cast<float*>(sm + C::kOffFc1);
+        float4* res = reinterpret_cast<float4*>(p.res + (size_t)blockIdx.x * kTowerResFloatsPerCta) + et;   // + k * 256
+        const float* hw = reinterpret_cast<const float*>(sm + C::kOffHw);
+        const float* ssh = p.ss + (size_t)L * 2 * F;   // folded BN of the head convolutions
+        uint32_t stage = 0, phase = 0, ss_buf = 0;
+        float d[128];
+        if (et < 2 * F) ss_s[et] = __ldg(p.ss + et);
+
+        for (uint32_t it = 0; it < iters; ++it) {
+            const uint32_t tile = blockIdx.x + it * gridDim.x;
+            const uint32_t pos0 = tile * B;
+            for (int idx = et; idx < 2 * 64 * B; idx += 256) {   // (row m, K-chunk pair) of the layer-0 im2col tile
+                const int m = idx & (64 * B - 1), g = m >> 3, brd = g % B;
+                const bool valid = pos0 + brd < p.n;
+                build_layer0_rows<C::kA0Kc>(sm + C::kOffA0, valid ? p.own[pos0 + brd] : 0, valid ? p.enemy[pos0 + brd] : 0,
+                                            2 * (idx / (64 * B)), g, m & 7, g / B);
+            }
+            fence_proxy_async();
+            for (int l = 0; l < L; ++l) {
+                const float* sc = ss_s + ss_buf * 2 * F;
+                const bool is_conv2 = l > 0 && (l & 1) == 0;
+                float4 rb[kResAhead];
+                epi_bar();
+                if (et < 2 * F) {
+                    const size_t nl = l + 1 < L ? (size_t)l + 1 : 0;
+                    cp_async_4(smem_u32(ss_s + (ss_buf ^ 1) * 2 * F + et), p.ss + nl * 2 * F + et);
+                }
+                acc_fence(d);
+                if (l == 0) {
+                    mbar_wait(bar_w0, 0);
+                    wgmma_fence();
+#pragma unroll
+                    for (uint32_t j = 0; j < 2; ++j)
+                        mma_kstep<F>(d, base + C::kOffA0 + j * 2 * C::kA0Kc + wg * T * 1024, 1024, C::kA0Kc, 128,
+                                     smem_desc(base + C::kOffW0 + j * 2 * F * 16, F * 16, 128), j);
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                } else {
+                    int prev = -1;
+                    for (int s = 0; s < C::S; ++s) {
+                        // stage s = taps (kh, kw0 .. kw0 + TPS - 1); tap (kh, kw) reads slot offset B*kh, chunk offset kw
+                        const int kh = C::TPS == 3 ? s : s / 3, kw0 = C::TPS == 3 ? 0 : s % 3;
+                        const uint32_t a_st = a_wg + B * kh * kActSlot + kw0 * 16;
+                        mbar_wait(bar_full(stage), phase);
+                        const uint32_t b_st = base + C::kOffW + stage * C::kStageBytes;
+                        wgmma_fence();
+#pragma unroll
+                        for (int ks = 0; ks < C::TPS * C::KPT; ++ks) {
+                            const int tt = ks / C::KPT, kk = ks % C::KPT;
+                            mma_kstep<F>(d, a_st + tt * 16 + 2 * kk * C::kActCg, 8 * kActSlot, C::kActCg, kActSlot,
+                                         smem_desc(b_st + tt * C::kTapBytes + 2 * kk * F * 16, F * 16, 128), (s | ks) != 0);
+                        }
+                        wgmma_commit();
+                        wgmma_wait<1>();
+                        if (prev >= 0 && lane == 0) {
+                            mbar_arrive(bar_empty(prev));
+                            if (CL > 1) mbar_arrive_cta(bar_empty(prev), crank ^ 1u);
+                        }
+                        prev = (int)stage;
+                        if (++stage == kStages) { stage = 0; phase ^= 1; }
+                    }
+                    if (is_conv2) {
+#pragma unroll
+                        for (int i = 0; i < kResAhead; ++i) rb[i] = res[i * 256];
+                    }
+                    wgmma_wait<0>();
+                    if (lane == 0) {
+                        mbar_arrive(bar_empty(prev));
+                        if (CL > 1) mbar_arrive_cta(bar_empty(prev), crank ^ 1u);
+                    }
+                }
+                acc_fence(d);
+                cp_async_wait_all();
+                ss_buf ^= 1;
+                const bool keep_res = l == 0 || is_conv2;
+                const bool last = l == L - 1;
+                if (!last) epi_bar();
+                // compiled once per layer kind (see rz_net_tc.cu); flat step k = t * F/8 + i covers channel 8i + cq of sub-tile t:
+                // accumulators d[4k .. 4k + 3], residual float4 k.  The last layer finishes sub-tile t's head 1x1 sums (and
+                // writes them to hp / hv) as soon as its channels are done, so that only six sums are live at a time.
+                constexpr int kEpiRelu = 0, kEpiKeep = 1, kEpiLast = 2;
+                auto epilogue = [&](auto conv2, auto kind) {
+                    constexpr bool kConv2 = decltype(conv2)::value;
+                    constexpr bool kKeep = decltype(kind)::value == kEpiKeep, kLast = decltype(kind)::value == kEpiLast;
+                    float hs[6];   // head sums (policy 0, policy 1, value) x (board b_t, b_t + 1) of the current sub-tile
+#pragma unroll
+                    for (int k = 0; k < 32; ++k) {
+                        const int t = k / (F / 8), c = 8 * (k % (F / 8)) + cq;
+                        if (kLast && c == cq) {
+#pragma unroll
+                            for (int h = 0; h < 6; ++h) hs[h] = 0.f;
+                        }
+                        const float2 s = *reinterpret_cast<const float2*>(sc + c);
+                        const float2 b = *reinterpret_cast<const float2*>(sc + F + c);
+                        float v0 = fmaf(d[4 * k + 0], s.x, b.x), v1 = fmaf(d[4 * k + 1], s.y, b.y);
+                        float v2 = fmaf(d[4 * k + 2], s.x, b.x), v3 = fmaf(d[4 * k + 3], s.y, b.y);
+                        if (kConv2) {
+                            const float4 r = rb[k % kResAhead];
+                            if (k + kResAhead < 32) rb[k % kResAhead] = res[(k + kResAhead) * 256];
+                            v0 += r.x; v1 += r.y; v2 += r.z; v3 += r.w;
+                        }
+                        if (kKeep || kLast) {
+                            v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); v2 = fmaxf(v2, 0.f); v3 = fmaxf(v3, 0.f);
+                        }
+                        if (!kLast) {
+                            if (kKeep) res[k * 256] = make_float4(v0, v1, v2, v3);
+                            const uint32_t h0 = pack_h2<!kKeep>(v0, v1);
+                            const uint32_t h1 = pack_h2<!kKeep>(v2, v3);
+                            const uint32_t off = t * 8 * kActSlot + (c >> 3) * C::kActCg;
+                            asm volatile("st.shared.b32 [%0], %1;" ::"r"(act_row0 + off), "r"(h0) : "memory");
+                            asm volatile("st.shared.b32 [%0], %1;" ::"r"(act_row0 + kActSlot + off), "r"(h1) : "memory");
+                        } else {
+                            const float4 w = *reinterpret_cast<const float4*>(hw + 2 * c);
+                            const float2 wv = *reinterpret_cast<const float2*>(hw + 2 * F + c);
+                            hs[0] = fmaf(v1, w.z, fmaf(v0, w.x, hs[0]));
+                            hs[1] = fmaf(v1, w.w, fmaf(v0, w.y, hs[1]));
+                            hs[2] = fmaf(v1, wv.y, fmaf(v0, wv.x, hs[2]));
+                            hs[3] = fmaf(v3, w.z, fmaf(v2, w.x, hs[3]));
+                            hs[4] = fmaf(v3, w.w, fmaf(v2, w.y, hs[4]));
+                            hs[5] = fmaf(v3, wv.y, fmaf(v2, wv.x, hs[5]));
+                            const int g = g0 + 8 * t, b = g % B, pix = (g / B) * 8 + x;
+                            if (p.dbg_tower) {
+                                if (pos0 + b < p.n)
+                                    *reinterpret_cast<float2*>(p.dbg_tower + ((size_t)(pos0 + b) * 64 + pix) * F + c) = make_float2(v0, v1);
+                                if (pos0 + b + 1 < p.n)
+                                    *reinterpret_cast<float2*>(p.dbg_tower + ((size_t)(pos0 + b + 1) * 64 + pix) * F + c) = make_float2(v2, v3);
+                            }
+                            if (c == F - 8 + cq) {   // sub-tile t done: the four lanes of a quad hold disjoint channel sets of its rows
+#pragma unroll
+                                for (int h = 0; h < 6; ++h) {
+                                    hs[h] += __shfl_xor_sync(0xffffffffu, hs[h], 1);
+                                    hs[h] += __shfl_xor_sync(0xffffffffu, hs[h], 2);
+                                }
+                                const int q = lane & 3;
+                                if (q < 2) {   // lane q of the quad: board b + q (BN + ReLU; Flatten is (C,H,W): index c*64 + pix)
+                                    hp[(b + q) * 128 + pix] = fmaxf(fmaf(q ? hs[3] : hs[0], ssh[0], ssh[2]), 0.f);
+                                    hp[(b + q) * 128 + 64 + pix] = fmaxf(fmaf(q ? hs[4] : hs[1], ssh[1], ssh[3]), 0.f);
+                                    hv[(b + q) * 64 + pix] = fmaxf(fmaf(q ? hs[5] : hs[2], ssh[4], ssh[5]), 0.f);
+                                }
+                            }
+                        }
+                    }
+                };
+                using Conv2 = std::true_type;
+                using NoConv2 = std::false_type;
+                if (last) {
+                    if (is_conv2) epilogue(Conv2(), std::integral_constant<int, kEpiLast>());
+                    else epilogue(NoConv2(), std::integral_constant<int, kEpiLast>());
+                } else if (is_conv2) {
+                    epilogue(Conv2(), std::integral_constant<int, kEpiKeep>());
+                } else if (keep_res) {
+                    epilogue(NoConv2(), std::integral_constant<int, kEpiKeep>());
+                } else {
+                    epilogue(NoConv2(), std::integral_constant<int, kEpiRelu>());
+                }
+                if (!last) fence_proxy_async();
+            }
+            // ---- heads (agent/model.py:43-56) for the B boards of the tile: hp / hv were written by the last epilogue ----
+            epi_bar();
+            for (int idx = et; idx < B * 64; idx += 256) {   // policy logits: Dense(128 -> 64)
+                const int b = idx >> 6, j = idx & 63;
+                const float* k = p.blob + p.off_policy_fc_k;
+                float acc = __ldg(p.blob + p.off_policy_fc_b + j);
+#pragma unroll 32
+                for (int i = 0; i < 128; ++i) acc = fmaf(hp[b * 128 + i], __ldg(k + i * 64 + j), acc);
+                logit[b * 64 + j] = acc;
+            }
+            for (int idx = et; idx < B * p.V; idx += 256) {   // value Dense(64 -> V) + ReLU
+                const int b = idx / p.V, j = idx - b * p.V;
+                const float* k = p.blob + p.off_value_fc1_k;
+                float acc = __ldg(p.blob + p.off_value_fc1_b + j);
+#pragma unroll 32
+                for (int i = 0; i < 64; ++i) acc = fmaf(hv[b * 64 + i], __ldg(k + (size_t)i * p.V + j), acc);
+                fc1[b * kTcMaxV + j] = fmaxf(acc, 0.f);
+            }
+            epi_bar();
+            for (int task = warp; task < 2 * B; task += 8) {
+                if (task < B) {   // softmax over 64 logits, one warp per board
+                    const int b = task;
+                    const float l0 = logit[b * 64 + lane], l1 = logit[b * 64 + 32 + lane];
+                    float mx = fmaxf(l0, l1);
+#pragma unroll
+                    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+                    const float e0 = expf(l0 - mx), e1 = expf(l1 - mx);
+                    float s = e0 + e1;
+#pragma unroll
+                    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+                    if (pos0 + b < p.n) {
+                        p.policy[(size_t)(pos0 + b) * 64 + lane] = e0 / s;
+                        p.policy[(size_t)(pos0 + b) * 64 + 32 + lane] = e1 / s;
+                        if (p.dbg_logits) {
+                            p.dbg_logits[(size_t)(pos0 + b) * 64 + lane] = l0;
+                            p.dbg_logits[(size_t)(pos0 + b) * 64 + 32 + lane] = l1;
+                        }
+                    }
+                } else {   // value Dense(V -> 1) + tanh, one warp per board
+                    const int b = task - B;
+                    float acc = 0.f;
+#pragma unroll 16
+                    for (int j = lane; j < p.V; j += 32) acc = fmaf(fc1[b * kTcMaxV + j], __ldg(p.blob + p.off_value_fc2_k + j), acc);
+#pragma unroll
+                    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+                    if (lane == 0 && pos0 + b < p.n) {
+                        const float pre = acc + __ldg(p.blob + p.off_value_fc2_b);
+                        p.value[pos0 + b] = tanhf(pre);
+                        if (p.dbg_vlogit) p.dbg_vlogit[pos0 + b] = pre;
+                    }
+                }
+            }
+        }
+    }
+
+    __syncthreads();
+    if (CL > 1) cluster_sync_all();
+}
+
+// ---- weight packing -----------------------------------------------------------------------------------
+template <int F>
+__global__ void pack_w0_narrow_kernel(const float* __restrict__ k0, __half* __restrict__ out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;   // over [4 kc][F n][8 j]
+    if (i >= 4 * F * 8) return;
+    const int j = i & 7, n = (i >> 3) % F, kc = i / (8 * F), k = kc * 8 + j;
+    out[i] = __float2half_rn(k < 18 ? k0[(size_t)k * F + n] : 0.f);   // conv0.kernel[kh][kw][c][n], K index = (kh*3+kw)*2 + c
+}
+// [layer][tap][F/8 kc][F n][8 j]: a stage is TPS consecutive taps
+template <int F>
+__global__ void pack_w_narrow_kernel(const float* __restrict__ blob, size_t off_res0, size_t stride, int n_layers, __half* __restrict__ out) {
+    const size_t total = (size_t)n_layers * 9 * F * F;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const int j = i & 7, n = (int)((i >> 3) % F), kc = (int)((i / (8 * F)) % (F / 8));
+        const size_t lt = i / ((size_t)F * F);
+        const int tap = (int)(lt % 9), l = (int)(lt / 9), ci = kc * 8 + j;
+        out[i] = __float2half_rn(blob[off_res0 + (size_t)l * stride + ((size_t)tap * F + ci) * F + n]);
+    }
+}
+
+template <int F>
+int pack(rz_net* net, cudaStream_t stream) {
+    pack_w0_narrow_kernel<F><<<(4 * F * 8 + 255) / 256, 256, 0, stream>>>(net->blob + net->off_conv0, net->tc_w0);
+    if (net->cfg.res_blocks > 0)
+        pack_w_narrow_kernel<F><<<num_sms() * 8, 256, 0, stream>>>(net->blob, net->off_res0, net->res_stride_conv, 2 * net->cfg.res_blocks, net->tc_w);
+    RZ_LAUNCH_CHECK();
+    return RZ_OK;
+}
+
+static std::mutex g_res_mutex;   // orders the launches that share a network's residual scratch
+
+template <int F>
+int launch(const Params& p, size_t n, cudaStream_t stream) {
+    using C = Cfg<F>;
+    static int max_pairs = -1;
+    if (max_pairs < 0) {
+        RZ_CUDA_TRY(cudaFuncSetAttribute(net_tower_narrow_kernel<F, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::kSmemAlloc));
+        RZ_CUDA_TRY(cudaFuncSetAttribute(net_tower_narrow_kernel<F, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::kSmemAlloc));
+        cudaLaunchConfig_t cfg = {};
+        cfg.gridDim = dim3((unsigned)num_sms() & ~1u); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = C::kSmemAlloc;
+        cudaLaunchAttribute attr[1];
+        attr[0].id = cudaLaunchAttributeClusterDimension;
+        attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+        cfg.attrs = attr; cfg.numAttrs = 1;
+        RZ_CUDA_TRY(cudaOccupancyMaxActiveClusters(&max_pairs, net_tower_narrow_kernel<F, 2>, &cfg));
+    }
+    const int cluster = tower_cluster() == 2 && max_pairs >= 1 ? 2 : 1;
+    const uint32_t ntiles = (uint32_t)((n + C::B - 1) / C::B);
+    uint32_t grid = ntiles < (uint32_t)num_sms() ? ntiles : (uint32_t)num_sms();
+    if (cluster == 1) {
+        net_tower_narrow_kernel<F, 1><<<grid, kThreads, C::kSmemAlloc, stream>>>(p);
+    } else {
+        grid = (grid + 1) & ~1u;   // whole clusters; a surplus CTA runs dummy tiles
+        if (grid > 2u * (uint32_t)max_pairs) grid = 2u * (uint32_t)max_pairs;
+        cudaLaunchConfig_t cfg = {};
+        cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = C::kSmemAlloc; cfg.stream = stream;
+        cudaLaunchAttribute attr[1];
+        attr[0].id = cudaLaunchAttributeClusterDimension;
+        attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+        cfg.attrs = attr; cfg.numAttrs = 1;
+        RZ_CUDA_TRY(cudaLaunchKernelEx(&cfg, net_tower_narrow_kernel<F, 2>, p));
+    }
+    RZ_LAUNCH_CHECK();
+    return RZ_OK;
+}
+
+}  // namespace narrow
+}  // namespace tc
+
+int net_pack_tc_narrow(rz_net* net, cudaStream_t stream) {
+    return net->cfg.filters == 128 ? tc::narrow::pack<128>(net, stream) : tc::narrow::pack<64>(net, stream);
+}
+
+int net_forward_tc_narrow(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value, size_t n, cudaStream_t stream,
+                          float* dbg_tower, const uint32_t* n_dev, float* dbg_logits, float* dbg_vlogit) {
+    const int F = net->cfg.filters;
+    RZ_REQUIRE(F == 64 || F == 128, "narrow wgmma tower requires 64 or 128 filters (got %d)", F);
+    RZ_REQUIRE(net->cfg.value_fc <= (int)tc::kTcMaxV, "wgmma tower supports value_fc_size <= %u", tc::kTcMaxV);
+    RZ_REQUIRE(n < (1ull << 31), "batch too large");
+    tc::Params p;
+    p.w0 = net->tc_w0; p.w = net->tc_w; p.ss = net->scale_shift; p.blob = net->blob;
+    p.off_policy_conv = net->off_policy_conv; p.off_policy_fc_k = net->off_policy_fc_k; p.off_policy_fc_b = net->off_policy_fc_b;
+    p.off_value_conv = net->off_value_conv; p.off_value_fc1_k = net->off_value_fc1_k; p.off_value_fc1_b = net->off_value_fc1_b;
+    p.off_value_fc2_k = net->off_value_fc2_k; p.off_value_fc2_b = net->off_value_fc2_b;
+    p.own = own; p.enemy = enemy; p.policy = policy; p.value = value; p.dbg_tower = dbg_tower;
+    p.dbg_logits = dbg_logits; p.dbg_vlogit = dbg_vlogit;
+    p.n = (uint32_t)n; p.n_dev = n_dev; p.n_layers = 1 + 2 * net->cfg.res_blocks; p.V = net->cfg.value_fc;
+    p.res = net->res;
+    std::lock_guard<std::mutex> lock(tc::narrow::g_res_mutex);
+    RZ_CUDA_TRY(cudaStreamWaitEvent(stream, net->res_done, 0));   // the previous launch on this scratch, whatever its stream
+    RZ_TRY(F == 128 ? tc::narrow::launch<128>(p, n, stream) : tc::narrow::launch<64>(p, n, stream));
+    RZ_CUDA_TRY(cudaEventRecord(net->res_done, stream));
+    return RZ_OK;
+}
+
+}  // namespace rz

@@ -112,6 +112,36 @@ __device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t adesc
         : "l"(adesc), "l"(bdesc), "r"(accumulate)
         : "memory");
 }
+// narrower N for the 64- / 128-filter tower (rz_net_tc_narrow.cu): D = d[O .. O + N/2 - 1] of the thread's 128 accumulators,
+// so that 256 / N such MMAs of one warpgroup (different A rows, the same B) fill the same register array
+template <int O>
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+        "}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+        : RZ_D16(O), RZ_D16(O + 16), RZ_D16(O + 32), RZ_D16(O + 48)
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
+        : "memory");
+}
+template <int O>
+__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+        "}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+        : RZ_D16(O), RZ_D16(O + 16)
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
+        : "memory");
+}
 #undef RZ_D16
 #undef RZ_D4
 

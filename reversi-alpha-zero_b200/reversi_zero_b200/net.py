@@ -6,6 +6,9 @@ import numpy as np
 from . import _cabi
 from .agent import model as M
 
+# AUTO: the tensor-core tower for 64-, 128- and 256-filter models with value_fc_size <= 512, else the fp32 generic kernel;
+# GENERIC: the exact fp32 path for any model; TCGEN05: the tensor-core tower (fp16 operands, fp32 accumulation);
+# SPLIT: the 256-filter tower split over 8-CTA clusters (same bits as TCGEN05)
 IMPL_AUTO, IMPL_GENERIC, IMPL_TCGEN05, IMPL_SPLIT = 0, 1, 2, 3
 
 
@@ -62,12 +65,15 @@ class Net:
                                                     stream_ptr), "rz_net_predict_dev")
 
     def debug_tower_dev(self, own_t, enemy_t, policy_t, value_t, tower_t, n, stream_ptr=None):
+        """tensor-core tower path that also writes the fp32 tower output: tower_t holds n * 64 * cnn_filter_num floats,
+        [position][pixel y*8+x][channel]"""
         _cabi.check(_cabi.lib().rz_net_debug_tower_dev(self._h, C.c_void_p(own_t.data_ptr()), C.c_void_p(enemy_t.data_ptr()),
                                                         C.c_void_p(policy_t.data_ptr()), C.c_void_p(value_t.data_ptr()),
                                                         C.c_void_p(tower_t.data_ptr()), n, stream_ptr), "rz_net_debug_tower_dev")
 
     def debug_heads_dev(self, own_t, enemy_t, policy_t, value_t, logits_t, vlogit_t, n, tower_t=None, stream_ptr=None):
-        """tensor-core tower path with the head outputs before softmax / tanh (and optionally the fp32 tower output)"""
+        """tensor-core tower path with the head outputs before softmax / tanh (and optionally the fp32 tower output,
+        sized as for debug_tower_dev)"""
         _cabi.check(_cabi.lib().rz_net_debug_heads_dev(self._h, C.c_void_p(own_t.data_ptr()), C.c_void_p(enemy_t.data_ptr()),
                                                         C.c_void_p(policy_t.data_ptr()), C.c_void_p(value_t.data_ptr()),
                                                         C.c_void_p(tower_t.data_ptr()) if tower_t is not None else None,
