@@ -352,7 +352,8 @@ int rz_ingest(const rz_play_row* rows, size_t n_rows, int save_policy_of_tau_1, 
  * Dense kernels; Keras SGD: v = momentum * v - lr * g, w = w + v for kernels, biases and BN gamma / beta; BN moving
  * statistics: moving = bn_momentum * moving + (1 - bn_momentum) * batch statistic.  3x3 convolutions use TF32 operands
  * with fp32 accumulation; every reduction has a fixed order, so equal inputs give bit-identical weights.
- * Configurations: filters a multiple of 16 in [16, 256], kernel_size 3, any res_blocks and value_fc (else RZ_EINVAL).
+ * Configurations: filters a multiple of 16 in [16, 256], kernel_size 3, res_blocks in [0, 64], value_fc in [1, 4096]
+ * (else RZ_EINVAL).
  * ---------------------------------------------------------------------------------------------- */
 typedef struct rz_trainer rz_trainer;
 
@@ -380,6 +381,26 @@ int rz_trainer_step_dev(rz_trainer* t, const uint8_t* planes, const float* polic
                         const int32_t* index, size_t batch, float lr, float* loss_dev, void* stream);
 /* test hook: gradient of the last step's total loss in blob layout (0 in the moving-statistics slots) */
 int rz_trainer_last_grad_dev(rz_trainer* t, float* grad_dev, size_t n_floats, void* stream);
+
+/* test hook: one of the step's 3x3-convolution GEMMs on caller buffers (device pointers, pixel-major [M = 64 * batch][C]),
+ * through the step's own kernels, weight images and weight-gradient split-K for this batch.  F = filters; kernels are in
+ * blob layout [9 taps = kh*3+kw][Cin][Cout]; bias [F] and add [M][F] are optional (NULL) where not required.
+ *   RZ_TRAIN_CONV0_FWD:   out[M][F] = conv(in[M][16], kernel[9][2][F]) + bias + add; in's channels 2..15 meet the zero
+ *                         padding of the weight image
+ *   RZ_TRAIN_CONV_FWD:    out[M][F] = conv(in[M][F], kernel[9][F][F]) + bias + add
+ *   RZ_TRAIN_CONV_DGRAD:  out[M][F] = input gradient of that convolution for dy = in (through the mirrored, transposed
+ *                         weight image) + bias + add; the step passes the skip connection's gradient as add
+ *   RZ_TRAIN_CONV_WGRAD:  out[9][F][F] = weight gradient for input in[M][F] and dy = add[M][F] (kernel and bias NULL)
+ *   RZ_TRAIN_CONV0_WGRAD: out[9][2][F] = the same for conv0's input in[M][16]
+ * Uses the trainer's scratch (the step rewrites it), so it must be stream-ordered with the steps; allocates nothing.
+ * RZ_EINVAL for batch outside [1, max_batch], a missing pointer or an unknown op. */
+#define RZ_TRAIN_CONV0_FWD 0
+#define RZ_TRAIN_CONV_FWD 1
+#define RZ_TRAIN_CONV_DGRAD 2
+#define RZ_TRAIN_CONV_WGRAD 3
+#define RZ_TRAIN_CONV0_WGRAD 4
+int rz_trainer_debug_conv_dev(rz_trainer* t, int op, const float* in, const float* kernel, const float* bias, const float* add,
+                              size_t batch, float* out, void* stream);
 
 #ifdef __cplusplus
 }

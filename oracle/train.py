@@ -45,6 +45,47 @@ class _Tf32Conv3x3(torch.autograd.Function):
         return gx, gk
 
 
+def _shift_rows(batch, device):
+    """src[tap][m]: the row that pixel m of a pixel-major [batch*64][C] tensor reads at tap = kh*3 + kw (offset
+    (kh-1, kw-1)), or batch*64 (a zero row) when that falls off the board"""
+    m = torch.arange(64 * batch, device=device)
+    y, x = (m % 64) // 8, m % 8
+    src = []
+    for tap in range(9):
+        yy, xx = y + tap // 3 - 1, x + tap % 3 - 1
+        ok = (yy >= 0) & (yy < 8) & (xx >= 0) & (xx < 8)
+        src.append(torch.where(ok, m - m % 64 + yy * 8 + xx, 64 * batch))
+    return src
+
+
+def _gather(x, src):
+    return torch.cat([x, x.new_zeros(1, x.shape[1])])[src]
+
+
+def conv3x3(x, k):
+    """the device trainer's convolution GEMMs restated as plain gathers and matrix products, in x's dtype and device.
+    x [B*64][Cin] pixel-major, k [9][Cin][Cout] (blob layout, tap = kh*3 + kw): out[m] = sum_tap x[shift(m, tap)] @ k[tap]"""
+    src = _shift_rows(x.shape[0] // 64, x.device)
+    return sum(_gather(x, src[t]) @ k[t] for t in range(9))
+
+
+def conv3x3_dgrad(dy, k):
+    """gradient of conv3x3 with respect to x for output gradient dy [B*64][Cout]: each tap's dy @ k[tap]^T added back to
+    the pixel it was read from"""
+    M = dy.shape[0]
+    src = _shift_rows(M // 64, dy.device)
+    out = dy.new_zeros(M + 1, k.shape[1])
+    for t in range(9):
+        out.index_add_(0, src[t], dy @ k[t].T)
+    return out[:M]
+
+
+def conv3x3_wgrad(x, dy):
+    """gradient of conv3x3 with respect to k: [9][Cin][Cout]"""
+    src = _shift_rows(x.shape[0] // 64, x.device)
+    return torch.stack([_gather(x, src[t]).T @ dy for t in range(9)])
+
+
 def is_trainable(name):
     return not (name.endswith(".bn_mean") or name.endswith(".bn_var"))
 

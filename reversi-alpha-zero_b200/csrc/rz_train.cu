@@ -915,4 +915,37 @@ int rz_trainer_last_grad_dev(rz_trainer* t, float* grad_dev, size_t n_floats, vo
     return RZ_OK;
 }
 
+int rz_trainer_debug_conv_dev(rz_trainer* t, int op, const float* in, const float* kernel, const float* bias, const float* add,
+                              size_t batch, float* out, void* stream) {
+    RZ_REQUIRE(t && in && out, "rz_trainer_debug_conv_dev: null pointer");
+    RZ_REQUIRE(batch >= 1 && batch <= (size_t)t->cfg.max_batch, "batch %zu outside [1, max_batch = %d]", batch, t->cfg.max_batch);
+    const int F = t->F, M = (int)batch * 64;
+    const cudaStream_t st = (cudaStream_t)stream;
+    RZ_CUDA_TRY(cudaSetDevice(t->device));
+    switch (op) {
+        case RZ_TRAIN_CONV0_FWD:
+            RZ_REQUIRE(kernel, "rz_trainer_debug_conv_dev: null kernel");
+            pack_w0_kernel<<<(9 * kCin0 * F + 255) / 256, 256, 0, st>>>(kernel, F, t->w0p);
+            RZ_LAUNCH_CHECK();
+            return launch_conv(in, kCin0, t->w0p, F, bias, add, out, M, st);
+        case RZ_TRAIN_CONV_FWD:
+            RZ_REQUIRE(kernel, "rz_trainer_debug_conv_dev: null kernel");
+            return launch_conv(in, F, kernel, F, bias, add, out, M, st);
+        case RZ_TRAIN_CONV_DGRAD:
+            RZ_REQUIRE(kernel, "rz_trainer_debug_conv_dev: null kernel");
+            pack_wt_kernel<<<grid_for((size_t)9 * F * F), 256, 0, st>>>(kernel, F, t->wt);
+            RZ_LAUNCH_CHECK();
+            return launch_conv(in, F, t->wt, F, bias, add, out, M, st);
+        case RZ_TRAIN_CONV_WGRAD:
+        case RZ_TRAIN_CONV0_WGRAD: {
+            RZ_REQUIRE(add && !kernel && !bias, "rz_trainer_debug_conv_dev: the weight gradient takes dy in `add`, no kernel or bias");
+            const bool c0 = op == RZ_TRAIN_CONV0_WGRAD;
+            return launch_wgrad(t, in, c0 ? kCin0 : F, c0 ? 2 : F, add, M, out, st);
+        }
+        default:
+            set_error("rz_trainer_debug_conv_dev: unknown op %d", op);
+            return RZ_EINVAL;
+    }
+}
+
 }  // extern "C"

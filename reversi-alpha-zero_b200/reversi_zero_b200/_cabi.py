@@ -121,6 +121,7 @@ SIGNATURES = {
     "rz_trainer_weights_dev": (C.c_int, [vp, vp, sz, vp]),
     "rz_trainer_step_dev": (C.c_int, [vp, vp, vp, vp, sz, vp, sz, C.c_float, vp, vp]),
     "rz_trainer_last_grad_dev": (C.c_int, [vp, vp, sz, vp]),
+    "rz_trainer_debug_conv_dev": (C.c_int, [vp, C.c_int, vp, vp, vp, vp, sz, vp, vp]),
 }
 
 _lib = None

@@ -16,6 +16,8 @@ from .agent import model as M
 
 MOMENTUM = 0.9      # SGD(momentum=0.9), worker/optimize.py:84
 BN_MOMENTUM = 0.99  # Keras BatchNormalization default
+# ops of Trainer.debug_conv (RZ_TRAIN_CONV* in include/rz_engine.h)
+CONV0_FWD, CONV_FWD, CONV_DGRAD, CONV_WGRAD, CONV0_WGRAD = 0, 1, 2, 3, 4
 
 
 class Trainer:
@@ -84,6 +86,22 @@ class Trainer:
         _cabi.check(_cabi.lib().rz_trainer_last_grad_dev(self._h, C.c_void_p(out.data_ptr()), out.numel(), self._stream()),
                     "rz_trainer_last_grad_dev")
         return out.cpu().numpy()
+
+    def debug_conv(self, op, x, batch, kernel=None, bias=None, add=None):
+        """test hook (rz_trainer_debug_conv_dev): one of the step's convolution GEMMs, CONV_* below, on float32 CUDA
+        tensors; x and add are [64 * batch][C], kernel [9][Cin][Cout].  Returns a new tensor: [64 * batch][F] for the
+        forward and input-gradient ops, the weight gradient [9][Cin][F] for the two WGRAD ops."""
+        import torch
+        F = self.mc.cnn_filter_num
+        for t in (x, kernel, bias, add):
+            if t is not None and (t.dtype != torch.float32 or not t.is_cuda or not t.is_contiguous()):
+                raise ValueError(f"expected a contiguous float32 CUDA tensor, got {t.dtype} on {t.device}")
+        shape = {CONV_WGRAD: (9, F, F), CONV0_WGRAD: (9, 2, F)}.get(op, (64 * batch, F))
+        out = torch.empty(shape, dtype=torch.float32, device=self.device)
+        ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
+        _cabi.check(_cabi.lib().rz_trainer_debug_conv_dev(self._h, op, ptr(x), ptr(kernel), ptr(bias), ptr(add), batch, ptr(out),
+                                                          self._stream()), "rz_trainer_debug_conv_dev")
+        return out
 
     def close(self):
         if self._h:

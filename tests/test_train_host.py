@@ -101,6 +101,23 @@ def test_tf32_rounding_and_format_model():
         assert 0 < err < 5e-2, (k, err)  # TF32's 2^-11 unit roundoff, amplified by the BN backward's cancellation
 
 
+@pytest.mark.parametrize("batch,cin,cout", [(1, 2, 16), (3, 48, 16), (2, 16, 80)])
+def test_conv_gemm_restatement_matches_torch(batch, cin, cout):
+    """oracle/train.py's gather-and-matmul convolutions (the reference of tests/test_train_shapes_gpu.py) are the
+    convolution, input gradient and weight gradient of F.conv2d(padding=1) on Keras-layout kernels"""
+    g = torch.Generator().manual_seed(batch * cin + cout)
+    x = torch.randn(batch, cin, 8, 8, generator=g, dtype=torch.float64)
+    k = torch.randn(3, 3, cin, cout, generator=g, dtype=torch.float64)
+    dy = torch.randn(batch, cout, 8, 8, generator=g, dtype=torch.float64)
+    kt = k.permute(3, 2, 0, 1)
+    pix = lambda t: t.permute(0, 2, 3, 1).reshape(-1, t.shape[1])   # NCHW -> [B*64][C]
+    ok = lambda a, b: torch.allclose(a, b, rtol=1e-12, atol=1e-12)
+    assert ok(ot.conv3x3(pix(x), k.reshape(9, cin, cout)), pix(F.conv2d(x, kt, padding=1)))
+    assert ok(ot.conv3x3_dgrad(pix(dy), k.reshape(9, cin, cout)), pix(torch.nn.grad.conv2d_input(x.shape, kt, dy, padding=1)))
+    assert ok(ot.conv3x3_wgrad(pix(x), pix(dy)),
+              torch.nn.grad.conv2d_weight(x, kt.shape, dy, padding=1).permute(2, 3, 1, 0).reshape(9, cin, cout))
+
+
 @pytest.mark.parametrize("filters,res,kernel,batch", [(24, 1, 3, 8), (8, 1, 3, 8), (272, 1, 3, 8), (16, 1, 5, 8), (16, 1, 3, 0)])
 def test_trainer_rejects_unsupported_configurations(filters, res, kernel, batch):
     ncfg = _cabi.NetCfg(filters, res, 8, kernel)
