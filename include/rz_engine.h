@@ -138,6 +138,10 @@ int rz_net_load_weights_dev(rz_net* net, const float* blob_dev, size_t n_floats,
  * policy[n][64] softmax probabilities, value[n] tanh.  Device pointers. */
 int rz_net_predict_dev(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value,
                        size_t n, int impl, void* stream);
+/* rz_net_predict_dev for a batch whose size is known only on the device: *count_dev (<= max_n) positions are evaluated,
+ * and rows from *count_dev to max_n of policy and value are left as they were (the engine's leaf-batch path). */
+int rz_net_predict_counted_dev(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value,
+                               const uint32_t* count_dev, size_t max_n, int impl, void* stream);
 /* diagnostic variant of the tensor-core tower path: additionally writes the fp32 residual-tower output
  * tower[n][64 pixels][filters channels] (pixel = y*8+x) so tests can localise a numerical difference. */
 int rz_net_debug_tower_dev(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value,

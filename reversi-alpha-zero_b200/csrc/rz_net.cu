@@ -291,7 +291,7 @@ int rz_net_destroy(rz_net* net) {
     if (!net) return RZ_OK;
     cudaSetDevice(net->device);
     cudaFree(net->blob); cudaFree(net->scale_shift); cudaFree(net->tc_w0); cudaFree(net->tc_w); cudaFree(net->scratch);
-    cudaFree(net->res);
+    cudaFree(net->res); cudaFree(net->feat);
     if (net->res_done) cudaEventDestroy(net->res_done);
     delete net;
     return RZ_OK;
@@ -325,6 +325,13 @@ int rz_net_predict_dev(rz_net* net, const uint64_t* own, const uint64_t* enemy, 
                        void* stream) {
     RZ_REQUIRE(net && (n == 0 || (own && enemy && policy && value)), "rz_net_predict_dev: null pointer");
     return net_forward(net, own, enemy, policy, value, n, impl, (cudaStream_t)stream);
+}
+
+int rz_net_predict_counted_dev(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value,
+                               const uint32_t* count_dev, size_t max_n, int impl, void* stream) {
+    RZ_REQUIRE(net && count_dev && (max_n == 0 || (own && enemy && policy && value)), "rz_net_predict_counted_dev: null pointer");
+    if (max_n == 0) return RZ_OK;
+    return net_forward_counted(net, own, enemy, policy, value, count_dev, max_n, impl, (cudaStream_t)stream);
 }
 
 int rz_net_debug_tower_dev(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value, float* tower, size_t n,

@@ -8,6 +8,7 @@
 //   scale = gamma / sqrt(var + 1e-3),  shift = beta + (bias - mean) * scale.
 #pragma once
 #include <cuda_fp16.h>
+#include <mutex>
 #include "rz_common.cuh"
 
 struct rz_net {
@@ -29,6 +30,10 @@ struct rz_net {
     // are ordered through res_done, recorded after every launch that uses it
     float* res;
     cudaEvent_t res_done;
+    // head features of the wgmma towers ([feat_rows][kHeadFeatures] fp32), grown on demand to a launch's batch capacity;
+    // shared by the launches of all streams like res, so ordered through res_done too
+    float* feat;
+    size_t feat_rows;
     // scratch for the host-buffer predict path
     void* scratch;
     size_t scratch_bytes;
@@ -37,6 +42,7 @@ struct rz_net {
 namespace rz {
 
 constexpr size_t kTowerResFloatsPerCta = 256 * 128;  // 128 KB: 256 math threads x 128 fp32 accumulators
+constexpr int kHeadFeatures = 192;                   // per board: policy head conv (2 x 64, Flatten order c*64 + pix), value (64)
 
 inline int n_conv_layers(const rz_net_cfg& c) { return 1 + 2 * c.res_blocks; }
 // per-layer folded BN parameters: scale at [l][0][*], shift at [l][1][*]
@@ -59,6 +65,11 @@ int net_forward_split(rz_net* net, const uint64_t* own, const uint64_t* enemy, f
 // RZ_NET_IMPL_AUTO -> the implementation used for a batch of capacity n
 int select_impl(const rz_net* net, size_t n, int impl);
 int net_pack_tc(rz_net* net, cudaStream_t stream);
+// the wgmma towers' launches on a network hold this lock: they share its residual scratch and head-feature buffer
+std::mutex& tower_mutex();
+// grows net->feat to at least n rows (under tower_mutex(); a reallocation synchronises the device first, since launches on
+// other streams may still read the old buffer)
+int head_features(rz_net* net, size_t n);
 // the same tower for 64 and 128 filters, B = 512 / F boards per tile (rz_net_tc_narrow.cu)
 int net_forward_tc_narrow(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value, size_t n,
                           cudaStream_t stream, float* dbg_tower, const uint32_t* n_dev, float* dbg_logits, float* dbg_vlogit);

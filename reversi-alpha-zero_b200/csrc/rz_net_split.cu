@@ -12,10 +12,10 @@
 //   * exchange: after a layer's MMAs a cluster barrier marks the operand buffers free; each CTA's epilogue (the same BN,
 //     skip and ReLU arithmetic) writes its 32-channel slice of the next operand into all 8 CTAs (st.shared::cluster); a
 //     second cluster barrier publishes it.  One operand buffer: two would not fit beside the weight ring;
-//   * residual stream: each thread keeps its 2 rows x 8 columns fp32 slice in registers (no global scratch, no ordering
-//     between launches, any number of concurrent streams);
-//   * heads: the fp32 tower output of the tile is gathered into CTA 0 (over the then idle operand buffer and weight ring),
-//     whose threads repeat the head sums of net_tower_kernel in its order (per lane over i = 0..31, then the lane quad).
+//   * residual stream: each thread keeps its 2 rows x 8 columns fp32 slice in registers (no global scratch);
+//   * head features: the fp32 tower output of the tile is gathered into CTA 0 (over the then idle operand buffer and weight
+//     ring), whose threads repeat the head sums of net_tower_kernel in its order (per lane over i = 0..31, then the lane
+//     quad) and store the same head features; the dense heads run afterwards in the batched head pass (rz_net_heads.cu).
 #include "rz_bitboard.cuh"
 #include "rz_net.cuh"
 #include "rz_tc_common.cuh"
@@ -36,12 +36,7 @@ constexpr uint32_t kOffAct = 0;
 constexpr uint32_t kOffW = kOffAct + kActBytes;
 constexpr uint32_t kOffA0 = kOffW + kStages * kSliceBytes;
 constexpr uint32_t kOffW0 = kOffA0 + kA0Bytes;
-constexpr uint32_t kOffPart = kOffW0 + kW0Bytes;         // [2][128][3]
-constexpr uint32_t kOffHp = kOffPart + 2 * 128 * 3 * 4;  // [2][128]
-constexpr uint32_t kOffHv = kOffHp + 2 * 128 * 4;        // [2][64]
-constexpr uint32_t kOffLogit = kOffHv + 2 * 64 * 4;      // [2][64]
-constexpr uint32_t kOffFc1 = kOffLogit + 2 * 64 * 4;     // [2][kTcMaxV]
-constexpr uint32_t kOffBar = kOffFc1 + 2 * kTcMaxV * 4;
+constexpr uint32_t kOffBar = kOffW0 + kW0Bytes;
 constexpr uint32_t kNumBars = 2 * kStages + 1;           // full[], empty[], w0
 constexpr uint32_t kSmemBytes = kOffBar + kNumBars * 8;
 constexpr uint32_t kSmemAlloc = kSmemBytes + 128;
@@ -210,7 +205,7 @@ __global__ void __cluster_dims__(kCluster, 1, 1) __launch_bounds__(kThreads, 1) 
     }
     if (crank != 0) return;   // no peer touches this CTA any more
 
-    // ---- heads on CTA 0, in the summation order of net_tower_kernel -------------------------------------
+    // ---- head features on CTA 0, in the summation order of net_tower_kernel ---------------------------
     const float* gat = reinterpret_cast<const float*>(sm);
     const float* pw = p.blob + p.off_policy_conv;
     const float* vw = p.blob + p.off_value_conv;
@@ -243,11 +238,10 @@ __global__ void __cluster_dims__(kCluster, 1, 1) __launch_bounds__(kThreads, 1) 
         hs[k] += __shfl_xor_sync(0xffffffffu, hs[k], 1);
         hs[k] += __shfl_xor_sync(0xffffffffu, hs[k], 2);
     }
-    const int q = lane & 3, brd = q & 1, m = r0 + 8 * brd;
-    const bool full = q < 2;
-    heads_phase(p, full ? hs[3 * brd] : 0.f, full ? hs[3 * brd + 1] : 0.f, full ? hs[3 * brd + 2] : 0.f, q >> 1, m, brd, y, x, et, warp,
-                lane, pos0, reinterpret_cast<float*>(sm + kOffPart), reinterpret_cast<float*>(sm + kOffHp),
-                reinterpret_cast<float*>(sm + kOffHv), reinterpret_cast<float*>(sm + kOffLogit), reinterpret_cast<float*>(sm + kOffFc1));
+    const int q = lane & 3;
+    if (q < 2 && pos0 + q < p.n)   // + 0.f as in net_tower_kernel
+        store_head_features(p.feat + (size_t)(pos0 + q) * kHeadFeatures, p.ss + (size_t)L * 512, y * 8 + x, hs[3 * q] + 0.f,
+                            hs[3 * q + 1] + 0.f, hs[3 * q + 2] + 0.f);
 }
 
 }  // namespace split
@@ -273,8 +267,14 @@ int net_forward_split(rz_net* net, const uint64_t* own, const uint64_t* enemy, f
     p.res = nullptr;
     const uint32_t ntiles = (uint32_t)((n + 1) / 2);
     if (ntiles == 0) return RZ_OK;
+    std::lock_guard<std::mutex> lock(tower_mutex());
+    RZ_TRY(head_features(net, n));
+    p.feat = net->feat;
+    RZ_CUDA_TRY(cudaStreamWaitEvent(stream, net->res_done, 0));   // the previous launch on the head-feature buffer
     split::net_split_kernel<<<ntiles * split::kCluster, split::kThreads, split::kSmemAlloc, stream>>>(p);
     RZ_LAUNCH_CHECK();
+    RZ_TRY(net_heads(p, stream));
+    RZ_CUDA_TRY(cudaEventRecord(net->res_done, stream));
     return RZ_OK;
 }
 

@@ -1,4 +1,4 @@
-// rz_net_tc.cu -- K4/K5: fused persistent wgmma residual tower + heads for the 256-filter network (sm_90a).
+// rz_net_tc.cu -- K4/K5: fused persistent wgmma residual tower + head features for the 256-filter network (sm_90a).
 //
 // One CTA per SM, each CTA owns a tile of TWO boards (M = 128 pixel rows) and carries it through the
 // WHOLE network without writing activations to HBM in between:
@@ -25,9 +25,11 @@
 //     (cp.async) into the idle half of a double buffer while the previous layer's MMAs run; the 1x1 head-conv weights
 //     are staged in shared memory once per CTA;
 //   * the first conv (2 -> 256 channels, K = 18 padded to 32) is a 2-MMA GEMM on an im2col tile built
-//     from the two bitboards; the policy / value heads run on the math warps from the fp32 tower
-//     output.
-// HBM traffic per position: 16 B in, 260 B out.  Algorithmic work: 2 * 755,343,616 flop (SURVEY 3.2).
+//     from the two bitboards; the last epilogue reduces the fp32 tower output to the 1x1 head convolutions and stores
+//     their BN + ReLU outputs (192 fp32 per board) for the dense heads, which run afterwards as one batched pass over
+//     all boards (rz_net_heads.cu) instead of once per tile on the math warps.
+// Global traffic per position: 16 B in and 768 B of head features out (the head pass reads them back and writes the
+// 260 B of policy and value).  Algorithmic work: 2 * 755,343,616 flop (SURVEY 3.2).
 #include <stdlib.h>
 #include <mutex>
 #include <type_traits>
@@ -55,12 +57,7 @@ constexpr uint32_t kOffA0 = kOffW + kStages * kStageBytes;
 constexpr uint32_t kOffW0 = kOffA0 + kA0Bytes;
 constexpr uint32_t kOffSS = kOffW0 + kW0Bytes;           // 2 x [scale 256][shift 256] fp32
 constexpr uint32_t kOffHw = kOffSS + 2 * 2048;           // 1x1 head-conv weights: policy [256][2], value [256] fp32
-constexpr uint32_t kOffPart = kOffHw + 768 * 4;          // [2 halves][128 rows][3] fp32 head partial sums
-constexpr uint32_t kOffHp = kOffPart + 2 * 128 * 3 * 4;  // [2 boards][128]
-constexpr uint32_t kOffHv = kOffHp + 2 * 128 * 4;        // [2][64]
-constexpr uint32_t kOffLogit = kOffHv + 2 * 64 * 4;      // [2][64]
-constexpr uint32_t kOffFc1 = kOffLogit + 2 * 64 * 4;     // [2][kTcMaxV]
-constexpr uint32_t kOffBar = kOffFc1 + 2 * kTcMaxV * 4;  // mbarriers
+constexpr uint32_t kOffBar = kOffHw + 768 * 4;           // mbarriers
 constexpr uint32_t kNumBars = 2 * kStages + 1;           // full[], empty[], w0
 constexpr uint32_t kSmemBytes = kOffBar + kNumBars * 8;
 constexpr uint32_t kSmemAlloc = kSmemBytes + 128;  // slack for manual 128 B alignment
@@ -73,7 +70,7 @@ static_assert(kTowerResFloatsPerCta == (size_t)kMathThreads * 128, "residual scr
 #ifdef RZ_TOWER_STAMPS
 enum : int {
     kStTiles,    // tiles processed (a count, not cycles)
-    kStTile,     // whole tile, layer-0 operand to the end of the heads
+    kStTile,     // whole tile, layer-0 operand to the last head-feature store
     kStKLoop,    // MMA sections of all layers: from the first weight wait to the last wgmma_wait
     kStFull,     // waiting on bar_full (weights late; the wgmmas already queued keep running meanwhile)
     kStMma,      // waiting in wgmma_wait (MMA-bound)
@@ -82,7 +79,7 @@ enum : int {
     kStEpi1,     // conv1 epilogues (first conv of a block)
     kStEpi2,     // conv2 epilogues (second conv of a block), except the last layer's
     kStEpiLast,  // last layer's epilogue (head 1x1 sums)
-    kStHeads,    // heads
+    kStFeat,     // head features: the 1x1 sums reduced over the lane quad, BN + ReLU, stored to global memory
     kStEmpty,    // producer: waiting on bar_empty (slot not yet released by both CTAs' math warps)
     kStCount
 };
@@ -176,11 +173,6 @@ __global__ void __launch_bounds__(kThreads, 1) net_tower_kernel(const Params pp)
         const uint32_t act_row1 = act_row0 + kActSlot;
         const uint32_t a_wg = base + kOffAct + wg * 8 * kActSlot;   // operand rows of this warpgroup, tap (0, 0)
         float* ss_s = reinterpret_cast<float*>(sm + kOffSS);
-        float* part = reinterpret_cast<float*>(sm + kOffPart);
-        float* hp = reinterpret_cast<float*>(sm + kOffHp);
-        float* hv = reinterpret_cast<float*>(sm + kOffHv);
-        float* logit = reinterpret_cast<float*>(sm + kOffLogit);
-        float* fc1 = reinterpret_cast<float*>(sm + kOffFc1);
         float4* res = reinterpret_cast<float4*>(p.res + (size_t)blockIdx.x * kTowerResFloatsPerCta) + et;   // + i * 256
         const float* hw = reinterpret_cast<const float*>(sm + kOffHw);
         uint32_t stage = 0, phase = 0, ss_buf = 0;
@@ -357,23 +349,27 @@ __global__ void __launch_bounds__(kThreads, 1) net_tower_kernel(const Params pp)
                 })
             }
             RZ_STAMP(const uint32_t st_h0 = (uint32_t)clock();)
-            // ---- heads (agent/model.py:43-56) on the 256 math threads ----------------------------------
-            // the four lanes of a row quad hold disjoint column sets of the same two rows
+            // ---- head features (agent/model.py:43-47) of the tile's two boards -----------------------------------
+            // the four lanes of a row quad hold disjoint column sets of the same two rows; lane q < 2 stores board q's features
 #pragma unroll
             for (int k = 0; k < 6; ++k) {
                 hs[k] += __shfl_xor_sync(0xffffffffu, hs[k], 1);
                 hs[k] += __shfl_xor_sync(0xffffffffu, hs[k], 2);
             }
-            // lane quad (0, 1, 2, 3) -> (row r0 colhalf 0, row r0 + 8 colhalf 0, r0 colhalf 1 = 0, r0 + 8 colhalf 1 = 0)
-            const int q = lane & 3, brd = q & 1, m = r0 + 8 * brd;
-            const bool full = q < 2;
-            // constant indices keep hs in registers (a lane-dependent index would put it in local memory)
-            const float h0 = brd ? hs[3] : hs[0], h1 = brd ? hs[4] : hs[1], h2 = brd ? hs[5] : hs[2];
-            heads_phase(p, full ? h0 : 0.f, full ? h1 : 0.f, full ? h2 : 0.f, q >> 1, m, brd, y, x, et,
-                        warp, lane, pos0, part, hp, hv, logit, fc1);
+            {
+                const int q = lane & 3;
+                if (q < 2 && pos0 + q < p.n) {
+                    // constant indices keep hs in registers (a lane-dependent index would put it in local memory).  The
+                    // + 0.f is the second column half's (zero) partial sum of the reduction these features were first
+                    // computed with; it turns a -0 sum into +0, and the outputs are held to those bits
+                    const float h0 = q ? hs[3] : hs[0], h1 = q ? hs[4] : hs[1], h2 = q ? hs[5] : hs[2];
+                    store_head_features(p.feat + (size_t)(pos0 + q) * kHeadFeatures, p.ss + (size_t)L * 512, y * 8 + x, h0 + 0.f,
+                                        h1 + 0.f, h2 + 0.f);
+                }
+            }
             RZ_STAMP(if (et == 0) {
                 const uint32_t st_h1 = (uint32_t)clock();
-                stamp_add(kStHeads, st_h1 - st_h0); stamp_add(kStTile, st_h1 - st_tile0); stamp_add(kStTiles, 1);
+                stamp_add(kStFeat, st_h1 - st_h0); stamp_add(kStTile, st_h1 - st_tile0); stamp_add(kStTiles, 1);
             })
         }
     }
@@ -411,7 +407,6 @@ int net_pack_tc(rz_net* net, cudaStream_t stream) {
     return RZ_OK;
 }
 
-static std::mutex g_res_mutex;   // orders the tower launches that share a network's residual scratch
 static int g_cluster = 0;        // 0: not yet decided (RZ_TOWER_CLUSTER, default 2)
 
 int set_tower_cluster(int cluster) {
@@ -458,7 +453,9 @@ int net_forward_tc(rz_net* net, const uint64_t* own, const uint64_t* enemy, floa
     p.dbg_logits = dbg_logits; p.dbg_vlogit = dbg_vlogit;
     p.n = (uint32_t)n; p.n_dev = n_dev; p.n_layers = 1 + 2 * net->cfg.res_blocks; p.V = net->cfg.value_fc;
     p.res = net->res;
-    std::lock_guard<std::mutex> lock(g_res_mutex);
+    std::lock_guard<std::mutex> lock(tower_mutex());
+    RZ_TRY(head_features(net, n));
+    p.feat = net->feat;
     RZ_CUDA_TRY(cudaStreamWaitEvent(stream, net->res_done, 0));   // the previous launch on this scratch, whatever its stream
     const uint32_t ntiles = (uint32_t)((n + 1) / 2);
     uint32_t grid = ntiles < (uint32_t)num_sms() ? ntiles : (uint32_t)num_sms();
@@ -476,6 +473,7 @@ int net_forward_tc(rz_net* net, const uint64_t* own, const uint64_t* enemy, floa
         RZ_CUDA_TRY(cudaLaunchKernelEx(&cfg, tc::net_tower_kernel<2>, p));
     }
     RZ_LAUNCH_CHECK();
+    RZ_TRY(net_heads(p, stream));
     RZ_CUDA_TRY(cudaEventRecord(net->res_done, stream));
     return RZ_OK;
 }

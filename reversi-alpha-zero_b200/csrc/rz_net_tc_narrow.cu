@@ -12,8 +12,9 @@
 //     producer thread (multicast across a CTA pair with CL = 2): one tap (32 KB, 9 stages per conv) at 128 filters, one
 //     kernel row of three taps (24 KB, 3 stages per conv) at 64 filters;
 //   * epilogue (folded BN, skip connection from the per-CTA fp32 residual scratch, ReLU, fp16 operand for the next layer),
-//     layer 0 (im2col GEMM, K = 18 padded to 32) and heads as in rz_net_tc.cu, for B boards.  A row's 1x1 head-conv sums
-//     are complete in its lane quad, so the heads need no cross-warpgroup partial-sum array.
+//     layer 0 (im2col GEMM, K = 18 padded to 32) and head features as in rz_net_tc.cu, for B boards.  A row's 1x1
+//     head-conv sums are complete in its lane quad, so they need no cross-warpgroup partial-sum array.  The dense heads
+//     run afterwards as one batched pass (rz_net_heads.cu).
 // Every output element goes through the same operations whichever tile slot its board lands in.
 #include <stdlib.h>
 #include <mutex>
@@ -53,11 +54,8 @@ struct Cfg {
     static constexpr uint32_t kOffW0 = kOffA0 + kA0Bytes;
     static constexpr uint32_t kOffSS = kOffW0 + kW0Bytes;           // 2 x [scale F][shift F] fp32
     static constexpr uint32_t kOffHw = kOffSS + 2 * 2 * F * 4;      // 1x1 head-conv weights: policy [F][2], value [F] fp32
-    static constexpr uint32_t kOffHp = kOffHw + 3 * F * 4;          // [B][128]
-    static constexpr uint32_t kOffHv = kOffHp + B * 128 * 4;        // [B][64]
-    static constexpr uint32_t kOffLogit = kOffHv + B * 64 * 4;      // [B][64]
-    static constexpr uint32_t kOffFc1 = kOffLogit + B * 64 * 4;     // [B][kTcMaxV]
-    static constexpr uint32_t kOffBar = kOffFc1 + B * kTcMaxV * 4;  // full[], empty[], w0
+    static constexpr uint32_t kOffFeat = kOffHw + 3 * F * 4;        // [B][kHeadFeatures] head features of the tile
+    static constexpr uint32_t kOffBar = kOffFeat + B * kHeadFeatures * 4;   // full[], empty[], w0
     static constexpr uint32_t kSmemBytes = kOffBar + (2 * kStages + 1) * 8;
     static constexpr uint32_t kSmemAlloc = kSmemBytes + 128;        // slack for manual 128 B alignment
     static_assert(kSmemAlloc <= 232448, "shared memory budget exceeded");
@@ -181,12 +179,9 @@ __global__ void __launch_bounds__(kThreads, 1) net_tower_narrow_kernel(const Par
         const uint32_t act_row0 = base + C::kOffAct + (g0 + B) * kActSlot + (x + 1) * 16 + cq * 2;  // + 8t*kActSlot + cg*kActCg
         const uint32_t a_wg = base + C::kOffAct + wg * T * 8 * kActSlot;                            // + 8t*kActSlot: sub-tile t
         float* ss_s = reinterpret_cast<float*>(sm + C::kOffSS);
-        float* hp = reinterpret_cast<float*>(sm + C::kOffHp);
-        float* hv = reinterpret_cast<float*>(sm + C::kOffHv);
-        float* logit = reinterpret_cast<float*>(sm + C::kOffLogit);
-        float* fc1 = reinterpret_cast<float*>(sm + C::kOffFc1);
         float4* res = reinterpret_cast<float4*>(p.res + (size_t)blockIdx.x * kTowerResFloatsPerCta) + et;   // + k * 256
         const float* hw = reinterpret_cast<const float*>(sm + C::kOffHw);
+        float* feat_s = reinterpret_cast<float*>(sm + C::kOffFeat);
         const float* ssh = p.ss + (size_t)L * 2 * F;   // folded BN of the head convolutions
         uint32_t stage = 0, phase = 0, ss_buf = 0;
         float d[128];
@@ -263,7 +258,7 @@ __global__ void __launch_bounds__(kThreads, 1) net_tower_narrow_kernel(const Par
                 if (!last) epi_bar();
                 // compiled once per layer kind (see rz_net_tc.cu); flat step k = t * F/8 + i covers channel 8i + cq of sub-tile t:
                 // accumulators d[4k .. 4k + 3], residual float4 k.  The last layer finishes sub-tile t's head 1x1 sums (and
-                // writes them to hp / hv) as soon as its channels are done, so that only six sums are live at a time.
+                // stores its head features) as soon as its channels are done, so that only six sums are live at a time.
                 constexpr int kEpiRelu = 0, kEpiKeep = 1, kEpiLast = 2;
                 auto epilogue = [&](auto conv2, auto kind) {
                     constexpr bool kConv2 = decltype(conv2)::value;
@@ -318,11 +313,9 @@ __global__ void __launch_bounds__(kThreads, 1) net_tower_narrow_kernel(const Par
                                     hs[h] += __shfl_xor_sync(0xffffffffu, hs[h], 2);
                                 }
                                 const int q = lane & 3;
-                                if (q < 2) {   // lane q of the quad: board b + q (BN + ReLU; Flatten is (C,H,W): index c*64 + pix)
-                                    hp[(b + q) * 128 + pix] = fmaxf(fmaf(q ? hs[3] : hs[0], ssh[0], ssh[2]), 0.f);
-                                    hp[(b + q) * 128 + 64 + pix] = fmaxf(fmaf(q ? hs[4] : hs[1], ssh[1], ssh[3]), 0.f);
-                                    hv[(b + q) * 64 + pix] = fmaxf(fmaf(q ? hs[5] : hs[2], ssh[4], ssh[5]), 0.f);
-                                }
+                                if (q < 2)   // lane q of the quad: board b + q
+                                    store_head_features(feat_s + (b + q) * kHeadFeatures, ssh, pix, q ? hs[3] : hs[0], q ? hs[4] : hs[1],
+                                                        q ? hs[5] : hs[2]);
                             }
                         }
                     }
@@ -341,57 +334,11 @@ __global__ void __launch_bounds__(kThreads, 1) net_tower_narrow_kernel(const Par
                 }
                 if (!last) fence_proxy_async();
             }
-            // ---- heads (agent/model.py:43-56) for the B boards of the tile: hp / hv were written by the last epilogue ----
+            // the tile's head features, staged in shared memory by the last epilogue (global stores there cost spills)
             epi_bar();
-            for (int idx = et; idx < B * 64; idx += 256) {   // policy logits: Dense(128 -> 64)
-                const int b = idx >> 6, j = idx & 63;
-                const float* k = p.blob + p.off_policy_fc_k;
-                float acc = __ldg(p.blob + p.off_policy_fc_b + j);
-#pragma unroll 32
-                for (int i = 0; i < 128; ++i) acc = fmaf(hp[b * 128 + i], __ldg(k + i * 64 + j), acc);
-                logit[b * 64 + j] = acc;
-            }
-            for (int idx = et; idx < B * p.V; idx += 256) {   // value Dense(64 -> V) + ReLU
-                const int b = idx / p.V, j = idx - b * p.V;
-                const float* k = p.blob + p.off_value_fc1_k;
-                float acc = __ldg(p.blob + p.off_value_fc1_b + j);
-#pragma unroll 32
-                for (int i = 0; i < 64; ++i) acc = fmaf(hv[b * 64 + i], __ldg(k + (size_t)i * p.V + j), acc);
-                fc1[b * kTcMaxV + j] = fmaxf(acc, 0.f);
-            }
-            epi_bar();
-            for (int task = warp; task < 2 * B; task += 8) {
-                if (task < B) {   // softmax over 64 logits, one warp per board
-                    const int b = task;
-                    const float l0 = logit[b * 64 + lane], l1 = logit[b * 64 + 32 + lane];
-                    float mx = fmaxf(l0, l1);
-#pragma unroll
-                    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-                    const float e0 = expf(l0 - mx), e1 = expf(l1 - mx);
-                    float s = e0 + e1;
-#pragma unroll
-                    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-                    if (pos0 + b < p.n) {
-                        p.policy[(size_t)(pos0 + b) * 64 + lane] = e0 / s;
-                        p.policy[(size_t)(pos0 + b) * 64 + 32 + lane] = e1 / s;
-                        if (p.dbg_logits) {
-                            p.dbg_logits[(size_t)(pos0 + b) * 64 + lane] = l0;
-                            p.dbg_logits[(size_t)(pos0 + b) * 64 + 32 + lane] = l1;
-                        }
-                    }
-                } else {   // value Dense(V -> 1) + tanh, one warp per board
-                    const int b = task - B;
-                    float acc = 0.f;
-#pragma unroll 16
-                    for (int j = lane; j < p.V; j += 32) acc = fmaf(fc1[b * kTcMaxV + j], __ldg(p.blob + p.off_value_fc2_k + j), acc);
-#pragma unroll
-                    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-                    if (lane == 0 && pos0 + b < p.n) {
-                        const float pre = acc + __ldg(p.blob + p.off_value_fc2_b);
-                        p.value[pos0 + b] = tanhf(pre);
-                        if (p.dbg_vlogit) p.dbg_vlogit[pos0 + b] = pre;
-                    }
-                }
+            if (pos0 < p.n) {
+                const uint32_t nf = (p.n - pos0 < (uint32_t)B ? p.n - pos0 : (uint32_t)B) * kHeadFeatures;
+                for (uint32_t i = et; i < nf; i += 256) p.feat[(size_t)pos0 * kHeadFeatures + i] = feat_s[i];
             }
         }
     }
@@ -428,8 +375,6 @@ int pack(rz_net* net, cudaStream_t stream) {
     RZ_LAUNCH_CHECK();
     return RZ_OK;
 }
-
-static std::mutex g_res_mutex;   // orders the launches that share a network's residual scratch
 
 template <int F>
 int launch(const Params& p, size_t n, cudaStream_t stream) {
@@ -488,9 +433,12 @@ int net_forward_tc_narrow(rz_net* net, const uint64_t* own, const uint64_t* enem
     p.dbg_logits = dbg_logits; p.dbg_vlogit = dbg_vlogit;
     p.n = (uint32_t)n; p.n_dev = n_dev; p.n_layers = 1 + 2 * net->cfg.res_blocks; p.V = net->cfg.value_fc;
     p.res = net->res;
-    std::lock_guard<std::mutex> lock(tc::narrow::g_res_mutex);
+    std::lock_guard<std::mutex> lock(tower_mutex());
+    RZ_TRY(head_features(net, n));
+    p.feat = net->feat;
     RZ_CUDA_TRY(cudaStreamWaitEvent(stream, net->res_done, 0));   // the previous launch on this scratch, whatever its stream
     RZ_TRY(F == 128 ? tc::narrow::launch<128>(p, n, stream) : tc::narrow::launch<64>(p, n, stream));
+    RZ_TRY(net_heads(p, stream));
     RZ_CUDA_TRY(cudaEventRecord(net->res_done, stream));
     return RZ_OK;
 }

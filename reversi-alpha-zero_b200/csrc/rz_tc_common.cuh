@@ -1,5 +1,5 @@
 // rz_tc_common.cuh -- PTX wrappers (mbarrier, bulk copy with cluster multicast, wgmma) and the pieces of the fused
-// tower kernel (rz_net_tc.cu) that do not depend on its pipeline: parameter block, layer-0 operand, heads.
+// tower kernel (rz_net_tc.cu) that do not depend on its pipeline: parameter block, layer-0 operand, head features.
 #pragma once
 #include <cuda_fp16.h>
 #include "rz_bitboard.cuh"
@@ -166,6 +166,7 @@ struct Params {
     float* policy;
     float* value;
     float* res;        // fp32 residual stream, [CTA][32][256 threads][4]
+    float* feat;       // head features, [n][kHeadFeatures]: written by the tower, read by the head pass
     float* dbg_tower;  // nullable
     float* dbg_logits; // nullable: [n][64] policy logits (before the softmax)
     float* dbg_vlogit; // nullable: [n] value before the tanh
@@ -204,79 +205,19 @@ __device__ __forceinline__ void build_layer0_operand(uint8_t* a0, u64 o, u64 e, 
     }
 }
 
-// heads (agent/model.py:43-56) on the 256 math threads of a CTA for its two boards: per-row partial sums of the 1x1 head
-// convolutions over two column halves (colhalf 0 / 1 of row m) -> BN + ReLU -> Dense(128 -> 64) + softmax,
-// Dense(64 -> V) + ReLU -> Dense(V -> 1) + tanh.  part [2][128][3], hp [2][128], hv [2][64], logit [2][64],
-// fc1 [2][kTcMaxV]: shared-memory scratch.  The Dense loops are unrolled far enough that each thread's weight loads
-// (L2 hits: the shared-memory carve-out leaves L1 too small to keep them) go out in a few large batches; the
-// summation order stays the loop order.
-__device__ __forceinline__ void heads_phase(const Params& p, float hp0, float hp1, float hvv, int colhalf, int m, int brd, int y, int x,
-                                            int et, int ew, int lane, uint32_t pos0, float* part, float* hp, float* hv, float* logit,
-                                            float* fc1) {
-    const float* ssh = p.ss + (size_t)p.n_layers * 512;
-    part[(colhalf * 128 + m) * 3 + 0] = hp0;
-    part[(colhalf * 128 + m) * 3 + 1] = hp1;
-    part[(colhalf * 128 + m) * 3 + 2] = hvv;
-    epi_bar();
-    if (colhalf == 0) {
-        const float a0 = part[m * 3 + 0] + part[(128 + m) * 3 + 0];
-        const float a1 = part[m * 3 + 1] + part[(128 + m) * 3 + 1];
-        const float av = part[m * 3 + 2] + part[(128 + m) * 3 + 2];
-        const int pix = y * 8 + x;
-        hp[brd * 128 + pix] = fmaxf(fmaf(a0, ssh[0], ssh[2]), 0.f);        // Flatten is (C,H,W): index c*64 + pix
-        hp[brd * 128 + 64 + pix] = fmaxf(fmaf(a1, ssh[1], ssh[3]), 0.f);
-        hv[brd * 64 + pix] = fmaxf(fmaf(av, ssh[4], ssh[5]), 0.f);
-    }
-    epi_bar();
-    if (et < 128) {  // policy logits: Dense(128 -> 64)
-        const int b = et >> 6, j = et & 63;
-        const float* k = p.blob + p.off_policy_fc_k;
-        float acc = __ldg(p.blob + p.off_policy_fc_b + j);
-#pragma unroll 32
-        for (int i = 0; i < 128; ++i) acc = fmaf(hp[b * 128 + i], __ldg(k + i * 64 + j), acc);
-        logit[b * 64 + j] = acc;
-    }
-    for (int idx = et; idx < 2 * p.V; idx += 256) {  // value Dense(64 -> V) + ReLU
-        const int b = idx / p.V, j = idx - b * p.V;
-        const float* k = p.blob + p.off_value_fc1_k;
-        float acc = __ldg(p.blob + p.off_value_fc1_b + j);
-#pragma unroll 32
-        for (int i = 0; i < 64; ++i) acc = fmaf(hv[b * 64 + i], __ldg(k + (size_t)i * p.V + j), acc);
-        fc1[b * kTcMaxV + j] = fmaxf(acc, 0.f);
-    }
-    epi_bar();
-    if (ew < 2) {  // softmax over 64 logits, one warp per board
-        const int b = ew;
-        const float l0 = logit[b * 64 + lane], l1 = logit[b * 64 + 32 + lane];
-        float mx = fmaxf(l0, l1);
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-        const float e0 = expf(l0 - mx), e1 = expf(l1 - mx);
-        float s = e0 + e1;
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-        if (pos0 + b < p.n) {
-            p.policy[(size_t)(pos0 + b) * 64 + lane] = e0 / s;
-            p.policy[(size_t)(pos0 + b) * 64 + 32 + lane] = e1 / s;
-            if (p.dbg_logits) {
-                p.dbg_logits[(size_t)(pos0 + b) * 64 + lane] = l0;
-                p.dbg_logits[(size_t)(pos0 + b) * 64 + 32 + lane] = l1;
-            }
-        }
-    } else if (ew < 4) {  // value Dense(V -> 1) + tanh, one warp per board
-        const int b = ew - 2;
-        float acc = 0.f;
-#pragma unroll 16
-        for (int j = lane; j < p.V; j += 32) acc = fmaf(fc1[b * kTcMaxV + j], __ldg(p.blob + p.off_value_fc2_k + j), acc);
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-        if (lane == 0 && pos0 + b < p.n) {
-            const float pre = acc + __ldg(p.blob + p.off_value_fc2_b);
-            p.value[pos0 + b] = tanhf(pre);
-            if (p.dbg_vlogit) p.dbg_vlogit[pos0 + b] = pre;
-        }
-    }
+// head features of one pixel of one board: BN + ReLU of its 1x1 head-conv sums (policy filters 0, 1 and value), stored
+// to the board's row f of the head-feature buffer in the Flatten (C,H,W) order of agent/model.py: policy c*64 + pix,
+// value 128 + pix.  The dense heads run on them afterwards, batched over all boards (rz_net_heads.cu).
+__device__ __forceinline__ void store_head_features(float* f, const float* ssh, int pix, float a0, float a1, float av) {
+    f[pix] = fmaxf(fmaf(a0, ssh[0], ssh[2]), 0.f);
+    f[64 + pix] = fmaxf(fmaf(a1, ssh[1], ssh[3]), 0.f);
+    f[128 + pix] = fmaxf(fmaf(av, ssh[4], ssh[5]), 0.f);
 }
 
 }  // namespace tc
+
+// the dense heads after a tower (rz_net_heads.cu): Dense(128 -> 64) + softmax and Dense(64 -> V) + ReLU -> Dense(V -> 1) +
+// tanh over p.feat for p.n boards (p.n_dev when set), many boards per CTA, on the tower's stream
+int net_heads(const tc::Params& p, cudaStream_t stream);
+
 }  // namespace rz

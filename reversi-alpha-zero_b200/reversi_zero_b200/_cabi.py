@@ -91,6 +91,7 @@ SIGNATURES = {
     "rz_net_load_weights": (C.c_int, [vp, f32p, sz]),
     "rz_net_load_weights_dev": (C.c_int, [vp, vp, sz, vp]),
     "rz_net_predict_dev": (C.c_int, [vp, vp, vp, vp, vp, sz, C.c_int, vp]),
+    "rz_net_predict_counted_dev": (C.c_int, [vp, vp, vp, vp, vp, vp, sz, C.c_int, vp]),
     "rz_net_set_tower_cluster": (C.c_int, [C.c_int]),
     "rz_net_debug_tower_dev": (C.c_int, [vp, vp, vp, vp, vp, vp, sz, vp]),
     "rz_net_debug_heads_dev": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, vp, sz, vp]),

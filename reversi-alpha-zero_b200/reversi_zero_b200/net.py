@@ -64,6 +64,14 @@ class Net:
                                                     C.c_void_p(policy_t.data_ptr()), C.c_void_p(value_t.data_ptr()), n, impl,
                                                     stream_ptr), "rz_net_predict_dev")
 
+    def predict_counted_dev(self, own_t, enemy_t, policy_t, value_t, count_t, max_n, impl=IMPL_AUTO, stream_ptr=None):
+        """predict_dev for the first count_t[0] (a uint32 on the device, <= max_n) of max_n positions, as the engine's
+        leaf batches run; the rows past the count are not written"""
+        _cabi.check(_cabi.lib().rz_net_predict_counted_dev(self._h, C.c_void_p(own_t.data_ptr()), C.c_void_p(enemy_t.data_ptr()),
+                                                            C.c_void_p(policy_t.data_ptr()), C.c_void_p(value_t.data_ptr()),
+                                                            C.c_void_p(count_t.data_ptr()), max_n, impl, stream_ptr),
+                    "rz_net_predict_counted_dev")
+
     def debug_tower_dev(self, own_t, enemy_t, policy_t, value_t, tower_t, n, stream_ptr=None):
         """tensor-core tower path that also writes the fp32 tower output: tower_t holds n * 64 * cnn_filter_num floats,
         [position][pixel y*8+x][channel]"""

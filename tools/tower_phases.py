@@ -26,7 +26,7 @@ sys.path.insert(0, PKG)
 
 # order of the kSt* enum in rz_net_tc.cu
 PHASES = ["tiles", "tile", "k_loop", "wait_bar_full", "wait_wgmma", "wait_epi_bar", "epilogue_layer0", "epilogue_conv1",
-          "epilogue_conv2", "epilogue_last", "heads", "producer_wait_bar_empty"]
+          "epilogue_conv2", "epilogue_last", "head_features", "producer_wait_bar_empty"]
 
 
 def build_stamped(out):
