@@ -349,6 +349,26 @@ int rz_ingest_dev(const rz_play_row* rows, size_t n_rows, int save_policy_of_tau
 int rz_ingest(const rz_play_row* rows, size_t n_rows, int save_policy_of_tau_1, int change_tau_turn,
               uint8_t* planes, float* policy, float* z);                       /* host pointers */
 
+/* play_*.json text -> the same three arrays, one output record per JSON record, in file order:
+ *   planes [n][2][8][8] uint8 = bit_to_array(own), bit_to_array(enemy); policy [n][64] and z [n] float32 =
+ *   float32(float64(text)) -- Python's correctly rounded float(), then round-to-nearest-even to float32.
+ * The text must be one JSON array of [[own, enemy], [p0, ..., p63], z] records: bitboards are integer literals in
+ * [0, 2^64) (refused otherwise, never truncated), the other 65 values JSON numbers or NaN / Infinity / -Infinity, any
+ * JSON whitespace between tokens.  Anything else -- a string, a wrong arity, a missing bracket, trailing bytes, a
+ * truncated file -- returns RZ_EINVAL with *error_offset = the byte offset of the first error (else (size_t)-1).
+ * *n_records is always set once the records are counted; if it exceeds `capacity` the call returns RZ_ECAPACITY and
+ * writes nothing, so a call with capacity 0 and null outputs sizes the buffers.
+ * rz_ingest_json_dev: text and outputs in device memory; runs on `stream` and synchronises it (the record count is
+ * read back to size the parse; records the device cannot round exactly are converted on the host and patched).
+ * rz_ingest_json_host: the host twin (same parser, host pointers).  rz_ingest_json: reads the file at `path`, host
+ * outputs, through the device parser (it reads the file twice when sized with capacity 0 first). */
+int rz_ingest_json_dev(const char* text, size_t n_bytes, size_t capacity, uint8_t* planes, float* policy, float* z,
+                       size_t* n_records, size_t* error_offset, void* stream);
+int rz_ingest_json_host(const char* text, size_t n_bytes, size_t capacity, uint8_t* planes, float* policy, float* z,
+                        size_t* n_records, size_t* error_offset);
+int rz_ingest_json(const char* path, size_t capacity, uint8_t* planes, float* policy, float* z, size_t* n_records,
+                   size_t* error_offset);
+
 /* ------------------------------------------------------------------------------------------------
  * Trainer -- one SGD step of the network on the device (worker/optimize.py:73-86 OptimizeWorker.train_epoch ->
  * Keras fit on agent/model.py:28-72,104-110).  Training-mode BatchNormalization (batch statistics, biased variance,

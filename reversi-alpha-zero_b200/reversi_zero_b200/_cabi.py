@@ -114,6 +114,9 @@ SIGNATURES = {
     "rz_read_play_rows": (C.c_int, [C.c_char_p, vp, sz, C.POINTER(sz), C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "rz_ingest_dev": (C.c_int, [vp, sz, C.c_int, C.c_int, vp, vp, vp, vp]),
     "rz_ingest": (C.c_int, [vp, sz, C.c_int, C.c_int, u8p, f32p, f32p]),
+    "rz_ingest_json_dev": (C.c_int, [vp, sz, sz, vp, vp, vp, C.POINTER(sz), C.POINTER(sz), vp]),
+    "rz_ingest_json_host": (C.c_int, [vp, sz, sz, vp, vp, vp, C.POINTER(sz), C.POINTER(sz)]),
+    "rz_ingest_json": (C.c_int, [C.c_char_p, sz, vp, vp, vp, C.POINTER(sz), C.POINTER(sz)]),
     "rz_trainer_create": (C.c_int, [C.POINTER(NetCfg), C.POINTER(TrainCfg), C.c_int, C.POINTER(vp)]),
     "rz_trainer_destroy": (C.c_int, [vp]),
     "rz_trainer_blob_size": (C.c_int, [vp, C.POINTER(sz)]),

@@ -6,6 +6,12 @@ training arrays on the device by ``rz_ingest`` (csrc/rz_ingest.cu).  No CPU fall
     rows, tau1, ctt = read_play_rows("data/play_data/play_20260922-101500.123456.rzrows")
     states, policy, z = to_training_arrays(rows, tau1, ctt)              # numpy, as the reference trainer holds them
     states_d, policy_d, z_d = to_training_tensors(rows, tau1, ctt, 0)    # torch tensors on cuda:0 for a device-side trainer
+
+and from the ``play_*.json`` text itself, parsed on the device by ``rz_ingest_json_dev`` (csrc/rz_ingest_json.cu), for
+play data without a rows twin (the reference's own self-play, or this engine with write_play_rows off):
+
+    states_d, policy_d, z_d = read_play_json("data/play_data/play_20260922-101500.123456.json", 0)
+    states, policy, z = read_play_json_host(path)                       # numpy, through the host twin of the parser
 """
 import ctypes as C
 import os
@@ -19,6 +25,7 @@ ROW_DTYPE = np.dtype([("own", "<u8"), ("enemy", "<u8"), ("n_visit", "<i4", (64,)
 assert ROW_DTYPE.itemsize == C.sizeof(_cabi.PlayRow) == 280
 
 ROWS_SUFFIX = ".rzrows"
+RZ_EINVAL, RZ_ECAPACITY = -1, -5   # include/rz_engine.h
 
 
 def rows_path_of(json_path):
@@ -78,6 +85,81 @@ def to_training_tensors(rows, save_policy_of_tau_1=True, change_tau_turn=4, devi
         _cabi.check(_cabi.lib().rz_ingest_dev(d_rows.data_ptr(), n, int(bool(save_policy_of_tau_1)), int(change_tau_turn), states.data_ptr(),
                                                policy.data_ptr(), z.data_ptr(), torch.cuda.current_stream().cuda_stream), "rz_ingest_dev")
     return states, policy, z
+
+
+class PlayJsonError(_cabi.RzError):
+    """A play_*.json file that is not an array of [[own, enemy], [p0..p63], z] records (truncated, for instance: the
+    reference's self-play writes its files in place); ``offset`` is the byte offset of the first error."""
+
+    def __init__(self, msg, offset):
+        super().__init__(msg)
+        self.offset = offset
+
+
+def _ingest_json(call, outputs, what):
+    """Runs ``call(capacity, pointers, n, off)`` twice -- once to count the records, once into outputs of that size --
+    and returns the three arrays; ``outputs(n)`` allocates them and returns (arrays, pointers)."""
+    n, off = C.c_size_t(), C.c_size_t()
+    rc = call(0, (None, None, None), n, off)
+    arrays = None
+    if rc == RZ_ECAPACITY:
+        arrays, ptrs = outputs(n.value)
+        rc = call(n.value, ptrs, n, off)
+    if rc == RZ_EINVAL and off.value != C.c_size_t(-1).value:
+        msg = _cabi.lib().rz_last_error()
+        raise PlayJsonError(f"{what}: {msg.decode() if msg else ''}", off.value)
+    _cabi.check(rc, what)
+    return arrays if arrays is not None else outputs(0)[0]
+
+
+def parse_play_json_host(text):
+    """Host twin of the device parser (same grammar and conversion, csrc/rz_json_parse.cuh): play_*.json bytes ->
+    (states uint8 [N,2,8,8], policy float32 [N,64], z float32 [N]) numpy arrays, one row per JSON record."""
+    text = bytes(text)
+    buf = C.create_string_buffer(text, len(text))
+
+    def outputs(n):
+        arrays = (np.empty((n, 2, 8, 8), np.uint8), np.empty((n, 64), np.float32), np.empty((n,), np.float32))
+        return arrays, tuple(a.ctypes.data for a in arrays)
+
+    def call(cap, ptrs, n, off):
+        return _cabi.lib().rz_ingest_json_host(buf, len(text), cap, *ptrs, C.byref(n), C.byref(off))
+
+    return _ingest_json(call, outputs, "rz_ingest_json_host")
+
+
+def read_play_json_host(path):
+    with open(path, "rb") as f:
+        return parse_play_json_host(f.read())
+
+
+def parse_play_json(text, device=0):
+    """play_*.json bytes -> (states, policy, z) torch tensors on cuda:``device``, parsed on the device by
+    rz_ingest_json_dev (csrc/rz_ingest_json.cu); what json.load + convert_to_training_data give, rounded to float32."""
+    import torch
+    dev = torch.device("cuda", device)
+    text = bytes(text)
+    with torch.cuda.device(dev):
+        d_text = torch.frombuffer(bytearray(text), dtype=torch.uint8).to(dev) if text else torch.empty(0, dtype=torch.uint8, device=dev)
+        stream = torch.cuda.current_stream().cuda_stream
+
+        def outputs(n):
+            arrays = (torch.empty((n, 2, 8, 8), dtype=torch.uint8, device=dev), torch.empty((n, 64), dtype=torch.float32, device=dev),
+                      torch.empty((n,), dtype=torch.float32, device=dev))
+            return arrays, tuple(a.data_ptr() for a in arrays)
+
+        def call(cap, ptrs, n, off):
+            return _cabi.lib().rz_ingest_json_dev(d_text.data_ptr() if len(text) else None, len(text), cap, *ptrs, C.byref(n),
+                                                  C.byref(off), stream)
+
+        return _ingest_json(call, outputs, "rz_ingest_json_dev")
+
+
+def read_play_json(path, device=0):
+    """A play_*.json file -> (states uint8 [N,2,8,8], policy float32 [N,64], z float32 [N]) tensors on cuda:``device``;
+    raises PlayJsonError (with the byte offset) if the file is malformed or incomplete."""
+    with open(path, "rb") as f:
+        return parse_play_json(f.read(), device)
 
 
 def load_play_data_dir(play_data_dir, device=0):

@@ -9,7 +9,9 @@ included, then a sleep of ``wait_after_save_model_ratio`` x the time since the l
 Differences, all on the data path:
   * the training data comes from the ``play_*.rzrows`` twin of every ``play_*.json`` (``b200.write_play_rows``), expanded
     on the device by ``rz_ingest_dev``; the JSON files hold policies rather than visit counts and cannot be converted, so
-    a JSON file whose twin does not appear stops the worker with a hint;
+    a JSON file whose twin does not appear stops the worker with a hint.  With ``b200.train_from_json`` the worker
+    instead parses every ``play_*.json`` itself on the device (``rz_ingest_json_dev``) and ignores the twins; as in the
+    reference, a file that does not parse (one still being written) is logged and retried at the next load;
   * each epoch runs ceil(N / batch_size) batches of a permutation drawn from the worker's own seeded generator (Keras uses
     numpy's global RNG);
   * a model is saved as ``next_generation/model_<ts>/model_weight.rzblob.npy`` only, built in a directory whose name does
@@ -78,14 +80,19 @@ class PerStepCallback:
 
 
 class OptimizeWorker:
-    def __init__(self, config, device=0, trainer=None, to_tensors=None, sleep=time.sleep, clock=time.time, seed=0):
-        """``trainer`` (an object with load_blob / step / blob, default ``train.Trainer``) and ``to_tensors`` (rows ->
-        (states, policy, z) tensors, default ``ingest.to_training_tensors`` on ``device``) can be replaced, e.g. by
+    def __init__(self, config, device=0, trainer=None, to_tensors=None, sleep=time.sleep, clock=time.time, seed=0,
+                 read_json=None):
+        """``trainer`` (an object with load_blob / step / blob, default ``train.Trainer``), ``to_tensors`` (rows ->
+        (states, policy, z) tensors, default ``ingest.to_training_tensors`` on ``device``) and ``read_json`` (a
+        play_*.json path -> the same tensors, default ``ingest.read_play_json`` on ``device``) can be replaced, e.g. by
         stand-ins in host-only tests."""
         self.config = config
         self.device = device
         self.trainer = trainer
         self.to_tensors = to_tensors or (lambda rows, tau1, ctt: ingest.to_training_tensors(rows, tau1, ctt, device))
+        self.read_json = read_json or (lambda path: ingest.read_play_json(path, device))
+        # the source of the training data: JSON can come from writers whose config this process cannot see
+        self.train_from_json = bool(getattr(getattr(config, "b200", None), "train_from_json", False))
         self.sleep, self.clock = sleep, clock
         self.seed = seed
         self.generator = None
@@ -221,6 +228,13 @@ class OptimizeWorker:
             self.dataset = self.collect_all_loaded_data()
 
     def load_data_from_file(self, filename):
+        if self.train_from_json:  # worker/optimize.py:182-189: a file that does not parse stays unloaded and is retried
+            try:
+                self.loaded_data[filename] = self.read_json(filename)
+                self.loaded_filenames.add(filename)
+            except Exception as e:
+                logger.warning(str(e))
+            return
         rows_path = ingest.rows_path_of(filename)
         if not os.path.exists(rows_path):
             first = self.missing_rows_since.setdefault(filename, self.clock())
