@@ -389,6 +389,20 @@ typedef struct rz_train_cfg {
 } rz_train_cfg;
 
 int rz_trainer_create(const rz_net_cfg* net, const rz_train_cfg* cfg, int device, rz_trainer** out);
+/* A data-parallel group of 1 <= n_devices <= 64 replicas on devices[0..n) (repeats allowed); devices[0] is the primary.
+ * Every rz_trainer_* call below takes either kind of handle, and a group's step gives exactly the bits of a single
+ * trainer's step on the same batch.  rz_trainer_step_dev splits the batch into contiguous shards, one per replica, whose
+ * boundaries sit on the weight-gradient split grid of the F->F convolutions (conv0's without residual blocks), as even
+ * as that grid allows (rz_train_shard_plan_host); a replica may get an empty shard.  Only the batch's own records leave
+ * the primary.  The replicas exchange per-record BatchNorm partials, per-record head tensors and weight-gradient split
+ * partials and add them in the single trainer's order; every replica then applies the same gradient, so weights,
+ * momentum and moving statistics stay identical.  The dataset, index, loss and stream are the primary's; the other
+ * replicas run on streams the trainer owns and join the caller's stream at the end of the step.  load_weights[_dev]
+ * load every replica; weights_dev, last_grad_dev and debug_conv_dev use the primary.  cfg->max_batch bounds the global
+ * batch.  n_devices == 1 is rz_trainer_create(devices[0]).  RZ_EINVAL for an ordinal outside the visible devices. */
+int rz_trainer_create_group(const rz_net_cfg* net, const rz_train_cfg* cfg, const int* devices, int n_devices, rz_trainer** out);
+/* the shards of a group step: replica r trains on batch positions [bounds[r], bounds[r + 1]); bounds has n_devices + 1 */
+int rz_train_shard_plan_host(int filters, int res_blocks, int batch, int n_devices, int32_t* bounds);
 int rz_trainer_destroy(rz_trainer* t);
 /* same count as rz_net_blob_size for the same configuration */
 int rz_trainer_blob_size(const rz_trainer* t, size_t* n_floats);
@@ -405,6 +419,9 @@ int rz_trainer_step_dev(rz_trainer* t, const uint8_t* planes, const float* polic
                         const int32_t* index, size_t batch, float lr, float* loss_dev, void* stream);
 /* test hook: gradient of the last step's total loss in blob layout (0 in the moving-statistics slots) */
 int rz_trainer_last_grad_dev(rz_trainer* t, float* grad_dev, size_t n_floats, void* stream);
+/* test hook: replica r's weights and momentum (blob layout) into blob_dev / vel_dev on the primary's device; r = 0 is the
+ * primary, and a single trainer has only replica 0 */
+int rz_trainer_replica_state_dev(rz_trainer* t, int r, float* blob_dev, float* vel_dev, size_t n_floats, void* stream);
 
 /* test hook: one of the step's 3x3-convolution GEMMs on caller buffers (device pointers, pixel-major [M = 64 * batch][C]),
  * through the step's own kernels, weight images and weight-gradient split-K for this batch.  F = filters; kernels are in

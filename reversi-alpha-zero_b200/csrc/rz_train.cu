@@ -10,6 +10,7 @@
 #include <string.h>
 #include <algorithm>
 #include <new>
+#include <type_traits>
 #include <vector>
 #include "rz_common.cuh"
 
@@ -233,6 +234,25 @@ __global__ void gather_kernel(const uint8_t* __restrict__ planes, const int32_t*
     x0[i] = c < 2 ? (float)planes[(size_t)r * 128 + c * 64 + p] : 0.f;
 }
 
+// a group's copy of the batch's own records in batch order (the replicas receive these, not the dataset), with the
+// substitution and *bad flag of gather_kernel: sp[b] = planes[index[b]], spol[b] = policy[index[b]], sz[b] = z[index[b]]
+__global__ void stage_kernel(const uint8_t* __restrict__ planes, const float* __restrict__ policy, const float* __restrict__ z,
+                             const int32_t* __restrict__ index, size_t n_records, int batch, uint8_t* __restrict__ sp,
+                             float* __restrict__ spol, float* __restrict__ sz, int* __restrict__ bad) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= batch * 64) return;
+    const int b = i >> 6, p = i & 63;
+    int32_t r = index[b];
+    if (r < 0 || (size_t)r >= n_records) {
+        if (p == 0) *bad = 1;
+        r = 0;
+    }
+    sp[(size_t)b * 128 + p] = planes[(size_t)r * 128 + p];
+    sp[(size_t)b * 128 + 64 + p] = planes[(size_t)r * 128 + 64 + p];
+    spol[(size_t)b * 64 + p] = policy[(size_t)r * 64 + p];
+    if (p == 0) sz[b] = z[r];
+}
+
 // ---- BatchNormalization (training mode) ------------------------------------------------------------------------------
 // Per-channel column reductions over the M = B*64 rows of a [M][ld] tensor (channels [0, C)): each CTA reduces 64 rows
 // into partial[chunk][v][C] (threads over channels x row lanes, lanes combined in order); a finalize kernel adds the
@@ -340,14 +360,15 @@ __global__ void bn_apply_kernel(const float* __restrict__ y, const float* __rest
 }
 
 // dy = gamma * invstd * (dz - (sum dz + xhat * sum dz*xhat) / M), dz = g where the layer's output is positive;
-// dz_out (nullable) keeps dz for the skip connection of a residual block
+// dz_out (nullable) keeps dz for the skip connection of a residual block.  Visits M rows; M_norm is the batch's row count
+// (M, except on a replica of a group, which holds a shard of the batch)
 __global__ void bn_backward_kernel(const float* __restrict__ g, const float* __restrict__ a, const float* __restrict__ y, int ld,
-                                   int C, int M, const float* __restrict__ blob, BnRef bn, const float* __restrict__ mean,
+                                   int C, int M, int M_norm, const float* __restrict__ blob, BnRef bn, const float* __restrict__ mean,
                                    const float* __restrict__ invstd, const float* __restrict__ sums, float* __restrict__ dy,
                                    float* __restrict__ dz_out) {
     const size_t total = (size_t)M * C;
     const float* gamma = blob + bn.off + bn.kf + bn.C;
-    const float inv_m = 1.f / (float)M;
+    const float inv_m = 1.f / (float)M_norm;
     for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
         const int c = (int)(i % C);
         const size_t o = (i / C) * ld + c;
@@ -609,6 +630,8 @@ __global__ void mask_grad_kernel(const float* __restrict__ grad, const uint8_t* 
 // dynamic shared memory of head_fc_kernel
 inline size_t head_fc_smem(int V) { return (size_t)(128 + 64 * 4 + 8 + 2 * V) * sizeof(double); }
 
+inline int chunks_of(int M) { return (M + kRowsPerChunk - 1) / kRowsPerChunk; }
+
 inline unsigned grid_for(size_t n, int threads = 256, size_t cap = 4096) {
     size_t b = (n + threads - 1) / threads;
     return (unsigned)(b < 1 ? 1 : b > cap ? cap : b);
@@ -639,10 +662,21 @@ struct rz_trainer {
     float *hc, *ah, *dh, *dyh;    // [M][3] head conv outputs, head BN+ReLU outputs, their gradients
     float *hp, *hv, *dl, *h1, *dh1, *dv, *lp, *lv;  // per-record head tensors
     float *stats;                 // [L + 2][4][F]: mean, invstd, sum dz, sum dz*xhat
-    double *part;                 // column-reduction partials [max_batch][3][F]
+    double *part;                 // column-reduction partials [max_batch][3][F] ([act][3][F] on replicas 1..)
     float *wpart;                 // weight-gradient split-K partials
     float *l2_part, *loss_pv;
     int* bad;
+    size_t act;                   // records the activation and backward buffers hold (max_batch for a single trainer)
+
+    // data-parallel group (rz_trainer_create_group): the handle is replica 0, the primary; a single trainer has none
+    std::vector<rz_trainer*> reps;  // every replica, reps[0] = this
+    cudaStream_t stream;          // replicas 1..: the stream the trainer owns (the primary runs on the caller's stream)
+    cudaEvent_t ev;               // marks this replica's progress at each exchange
+    uint8_t* sp;                  // staged batch records: planes [.][128], policy [.][64], z [.] (primary: max_batch)
+    float *spol, *sz;
+    int32_t* iota;                // identity index [act]: the staged records are the replica's dataset
+    float* wgather;               // primary: every layer's weight-gradient split partials [L][wslot], reduced after the join
+    size_t wslot;
 };
 
 namespace {
@@ -650,17 +684,52 @@ namespace {
 void trainer_free(rz_trainer* t) {
     float* bufs[] = {t->blob, t->vel, t->grad, t->stat, t->x0, t->w0p, t->wt, t->y, t->a, t->g, t->g1, t->dy, t->dz, t->hc, t->ah,
                      t->dh, t->dyh, t->hp, t->hv, t->dl, t->h1, t->dh1, t->dv, t->lp, t->lv, t->stats, t->wpart,
-                     t->l2_part, t->loss_pv};
+                     t->l2_part, t->loss_pv, t->spol, t->sz, t->wgather};
     for (float* p : bufs) cudaFree(p);
     cudaFree(t->part);
     cudaFree(t->kind);
     cudaFree(t->bad);
+    cudaFree(t->sp);
+    cudaFree(t->iota);
+    if (t->stream) cudaStreamDestroy(t->stream);
+    if (t->ev) cudaEventDestroy(t->ev);
 }
 
 int wgrad_splits(int cin, int F, int batch) {
     const int tiles = ((9 * cin + kBM - 1) / kBM) * ((F + kBN - 1) / kBN);
     int s = (kWgradTargetBlocks + tiles - 1) / tiles;
     return s < batch ? s : batch;
+}
+
+// records per weight-gradient split of a convolution with cin input channels (launch_wgrad)
+int wgrad_per(int cin, int F, int batch) {
+    const int splits = wgrad_splits(cin, F, batch);
+    return (batch + splits - 1) / splits;
+}
+
+// Shards of a group step: replica r trains on records [bounds[r], bounds[r + 1]).  The boundaries sit on the weight-
+// gradient split grid of the F->F convolutions (conv0's grid without residual blocks), so every split of those layers
+// lies inside one shard; the grid's cells are dealt out as evenly as possible, the larger shares first.
+void shard_plan(int F, int R, int batch, int n, int* bounds) {
+    const int per = wgrad_per(R ? F : kCin0, F, batch), cells = (batch + per - 1) / per;
+    const int q = cells / n, rem = cells % n;
+    for (int r = 0; r <= n; ++r) bounds[r] = std::min(batch, per * (r * q + std::min(r, rem)));
+}
+
+// conv0's weight-gradient splits are finer than the tower's and may straddle the end of a shard: a replica computes the
+// splits that start in its shard, which takes the first `ov` records of the next shard as well
+struct Conv0Share {
+    int z0, nz;         // its conv0 splits [z0, z0 + nz)
+    int row0, rows;     // the records they cover, relative to the shard's first
+    int ov;             // records past the end of the shard (rows of the next replica)
+};
+
+Conv0Share conv0_share(int F, int batch, int b0, int n) {
+    if (n == 0) return Conv0Share{0, 0, 0, 0, 0};
+    const int per0 = wgrad_per(kCin0, F, batch), e = b0 + n;
+    const int z0 = (b0 + per0 - 1) / per0, z1 = (e + per0 - 1) / per0;
+    const int end = std::min(z1 * per0, batch);
+    return z1 > z0 ? Conv0Share{z0, z1 - z0, z0 * per0 - b0, end - z0 * per0, end - e} : Conv0Share{z0, 0, 0, 0, 0};
 }
 
 int launch_conv(const float* in, int cin, const float* w, int F, const float* bias, const float* add, float* out, int M,
@@ -702,13 +771,13 @@ void bn_backward(rz_trainer* t, const float* gp, const float* ap, const float* y
     float *mean = st4, *invstd = st4 + t->F, *sums = st4 + 2 * t->F;
     colred_partial_kernel<kBnGrad><<<chunks, 256, 0, st>>>(yp, ap, gp, ld, 0, C, M, mean, invstd, t->part);
     colred_finalize_kernel<kBnGrad><<<1, 256, 0, st>>>(t->part, chunks, C, M, bn, mean, invstd, sums, t->stat, t->grad);
-    bn_backward_kernel<<<grid_for((size_t)M * C), 256, 0, st>>>(gp, ap, yp, ld, C, M, t->blob, bn, mean, invstd, sums, dyp, dz_out);
+    bn_backward_kernel<<<grid_for((size_t)M * C), 256, 0, st>>>(gp, ap, yp, ld, C, M, M, t->blob, bn, mean, invstd, sums, dyp, dz_out);
 }
 
 int trainer_step(rz_trainer* t, const uint8_t* planes, const float* policy, const float* z, const int32_t* index, size_t n_records,
                  int batch, float lr, float* loss, cudaStream_t st) {
     const int F = t->F, R = t->R, L = t->L, V = t->V, M = batch * 64;
-    const size_t MF = (size_t)M * F, lstride = (size_t)64 * t->cfg.max_batch * F;
+    const size_t MF = (size_t)M * F, lstride = (size_t)64 * t->act * F;
     auto Y = [&](int l) { return t->y + (size_t)l * lstride; };
     auto A = [&](int l) { return t->a + (size_t)l * lstride; };
     auto ST = [&](int l) { return t->stats + (size_t)l * 4 * F; };
@@ -775,12 +844,307 @@ int trainer_step(rz_trainer* t, const uint8_t* planes, const float* policy, cons
     return RZ_OK;
 }
 
-}  // namespace
+// ---- data-parallel group step ----------------------------------------------------------------------------------------
+// The step of trainer_step with the batch split into the shards of shard_plan, one per replica, and the same operations
+// in the same order on every sum the one-device step takes over the batch:
+//  * column reductions (BN statistics, BN and head-conv gradients): every replica writes the per-record partials of its
+//    shard; the primary gathers them into its `part` in batch order and runs the finalize over all chunks with the global
+//    M; the replicas copy back the finalized mean / invstd / sums (and the batch statistics of the moving averages);
+//  * dense heads: the per-record head tensors are gathered on the primary, which runs head_fc_grad_kernel on the batch;
+//  * weight gradients: every replica computes the split-K partials of its own splits (conv0's straddling split with the
+//    next replica's first rows); the primary gathers them into one slot per layer and reduces every layer in split order;
+//  * the primary then hands its whole gradient and the `bad` flag to every replica, and every replica runs update_kernel
+//    on them, so weights, momentum and moving statistics stay identical without a weight broadcast.
+// Transport is cudaMemcpyPeerAsync (a device-to-device copy between replicas on one device) ordered by one event per
+// replica.  At every exchange the primary waits on every replica (empty ones included), and the exchange ends with every
+// replica waiting on the primary, so no buffer a copy reads is rewritten before the copy has run; the replicas join the
+// caller's stream at the end and wait on it at the start.  A replica with an empty shard launches nothing but its copy
+// of the moving-average statistics, the gradient copy and update_kernel.
+int group_step(rz_trainer* t, const uint8_t* planes, const float* policy, const float* z, const int32_t* index, size_t n_records,
+               int batch, float lr, float* loss, cudaStream_t st) {
+    const int F = t->F, R = t->R, L = t->L, V = t->V, n = (int)t->reps.size(), Mg = batch * 64;
+    int bounds[65];
+    shard_plan(F, R, batch, n, bounds);
+    const int per = wgrad_per(R ? F : kCin0, F, batch), per0 = wgrad_per(kCin0, F, batch);
+    auto on = [&](int r) { return cudaSetDevice(t->reps[r]->device); };
+    auto S = [&](int r) { return r ? t->reps[r]->stream : st; };
+    auto b0 = [&](int r) { return bounds[r]; };
+    auto nr = [&](int r) { return bounds[r + 1] - bounds[r]; };
+    auto Y = [&](rz_trainer* p, int l) { return p->y + (size_t)l * 64 * p->act * F; };
+    auto A = [&](rz_trainer* p, int l) { return p->a + (size_t)l * 64 * p->act * F; };
+    auto ST = [&](rz_trainer* p, int l) { return p->stats + (size_t)l * 4 * F; };
+    auto bnref = [&](int l) { return BnRef{t->conv_off[l], (size_t)9 * (l ? F : 2) * F, F}; };
+    auto peer = [&](void* dst, int r_dst, const void* src, int r_src, size_t bytes, cudaStream_t s) {
+        return bytes ? cudaMemcpyPeerAsync(dst, t->reps[r_dst]->device, src, t->reps[r_src]->device, bytes, s) : cudaSuccess;
+    };
+    const int chunks = batch;  // kRowsPerChunk = 64 rows: one column-reduction partial per record
+    // the capacities rz_trainer_create_group computed: a shard and its conv0 overflow fit the replica's buffers, and
+    // every layer's split partials fit one gradient slot
+    for (int r = 0; r < n; ++r)
+        RZ_REQUIRE((size_t)nr(r) + conv0_share(F, batch, b0(r), nr(r)).ov <= t->reps[r]->act,
+                   "group step: shard of replica %d exceeds its buffers", r);
+    RZ_REQUIRE((size_t)((batch + per - 1) / per) * 9 * (R ? F : kCin0) * F <= t->wslot &&
+                   (size_t)((batch + per0 - 1) / per0) * 9 * kCin0 * F <= t->wslot,
+               "group step: weight-gradient splits exceed the gradient slot");
 
-extern "C" {
+    // stage the batch on the primary; each replica copies its shard (and conv0's overflow records) and expands x0
+    RZ_CUDA_TRY(cudaMemsetAsync(t->bad, 0, sizeof(int), st));
+    stage_kernel<<<(Mg + 255) / 256, 256, 0, st>>>(planes, policy, z, index, n_records, batch, t->sp, t->spol, t->sz, t->bad);
+    RZ_LAUNCH_CHECK();
+    RZ_CUDA_TRY(cudaEventRecord(t->ev, st));
+    for (int r = 0; r < n; ++r) {
+        rz_trainer* p = t->reps[r];
+        const cudaStream_t s = S(r);
+        RZ_CUDA_TRY(on(r));
+        const int rows = nr(r) + (R ? conv0_share(F, batch, b0(r), nr(r)).ov : 0);
+        if (r) {
+            RZ_CUDA_TRY(cudaStreamWaitEvent(s, t->ev, 0));
+            RZ_CUDA_TRY(peer(p->sp, r, t->sp + (size_t)b0(r) * 128, 0, (size_t)rows * 128, s));
+            RZ_CUDA_TRY(peer(p->spol, r, t->spol + (size_t)b0(r) * 64, 0, (size_t)rows * 64 * sizeof(float), s));
+            RZ_CUDA_TRY(peer(p->sz, r, t->sz + b0(r), 0, (size_t)rows * sizeof(float), s));
+        }
+        if (!nr(r)) continue;
+        gather_kernel<<<(rows * 64 * kCin0 + 255) / 256, 256, 0, s>>>(p->sp, p->iota, p->act, rows, p->x0, p->bad);
+        pack_w0_kernel<<<(9 * kCin0 * F + 255) / 256, 256, 0, s>>>(p->blob + t->conv_off[0], F, p->w0p);
+        for (int l = 1; l < L; ++l)
+            pack_wt_kernel<<<grid_for((size_t)9 * F * F), 256, 0, s>>>(p->blob + t->conv_off[l], F, p->wt + (size_t)(l - 1) * 9 * F * F);
+        RZ_LAUNCH_CHECK();
+    }
 
-int rz_trainer_create(const rz_net_cfg* net, const rz_train_cfg* cfg, int device, rz_trainer** out) {
-    RZ_REQUIRE(net && cfg && out, "rz_trainer_create: null pointer");
+    // the replicas' partials of `rec` doubles per record go to the primary's `part` in batch order
+    auto gather_part = [&](size_t rec) -> int {
+        for (int r = 1; r < n; ++r) {
+            RZ_CUDA_TRY(on(r));
+            RZ_CUDA_TRY(cudaEventRecord(t->reps[r]->ev, S(r)));
+        }
+        RZ_CUDA_TRY(on(0));
+        for (int r = 1; r < n; ++r) {
+            RZ_CUDA_TRY(cudaStreamWaitEvent(st, t->reps[r]->ev, 0));
+            if (!nr(r)) continue;
+            RZ_CUDA_TRY(peer(t->part + (size_t)b0(r) * rec, 0, t->reps[r]->part, r, (size_t)nr(r) * rec * sizeof(double), st));
+        }
+        return RZ_OK;
+    };
+    // after the primary's finalize: the replicas wait for it and copy layer l's finalized statistics (those with an empty
+    // shard never read them) and the `stat_n` moving-average batch statistics at stat_off (which update_kernel reads)
+    auto release = [&](int l, size_t stat_off, size_t stat_n) -> int {
+        RZ_CUDA_TRY(on(0));
+        RZ_CUDA_TRY(cudaEventRecord(t->ev, st));
+        for (int r = 1; r < n; ++r) {
+            rz_trainer* p = t->reps[r];
+            RZ_CUDA_TRY(on(r));
+            RZ_CUDA_TRY(cudaStreamWaitEvent(p->stream, t->ev, 0));
+            if (l >= 0 && nr(r)) RZ_CUDA_TRY(peer(ST(p, l), r, ST(t, l), 0, (size_t)4 * F * sizeof(float), p->stream));
+            RZ_CUDA_TRY(peer(p->stat + stat_off, r, t->stat + stat_off, 0, stat_n * sizeof(float), p->stream));
+        }
+        return RZ_OK;
+    };
+    // launch(r, replica, rows, stream) on every replica with a non-empty shard
+    auto partial_each = [&](auto launch) -> int {
+        for (int r = 0; r < n; ++r) {
+            if (!nr(r)) continue;
+            RZ_CUDA_TRY(on(r));
+            if constexpr (std::is_void_v<decltype(launch(r, t, 0, st))>) launch(r, t->reps[r], nr(r) * 64, S(r));
+            else RZ_TRY(launch(r, t->reps[r], nr(r) * 64, S(r)));
+            RZ_LAUNCH_CHECK();
+        }
+        return RZ_OK;
+    };
+    // training-mode BN forward of layer slot l: yp(p) [rows][ld], res(p) nullable, out(p)
+    auto bn_forward_g = [&](auto yp, auto res, int ld, int C, BnRef bn, int l, auto out) -> int {
+        RZ_TRY(partial_each([&](int, rz_trainer* p, int M, cudaStream_t s) {
+            colred_partial_kernel<kSum><<<chunks_of(M), 256, 0, s>>>(yp(p), nullptr, nullptr, ld, 0, C, M, nullptr, nullptr, p->part);
+        }));
+        RZ_TRY(gather_part(C));
+        colred_finalize_kernel<kSum><<<1, 256, 0, st>>>(t->part, chunks, C, Mg, bn, ST(t, l), ST(t, l) + F, nullptr, t->stat, t->grad);
+        RZ_LAUNCH_CHECK();
+        RZ_TRY(release(l, 0, 0));
+        RZ_TRY(partial_each([&](int, rz_trainer* p, int M, cudaStream_t s) {
+            colred_partial_kernel<kSqDev><<<chunks_of(M), 256, 0, s>>>(yp(p), nullptr, nullptr, ld, 0, C, M, ST(p, l), nullptr, p->part);
+        }));
+        RZ_TRY(gather_part(C));
+        colred_finalize_kernel<kSqDev><<<1, 256, 0, st>>>(t->part, chunks, C, Mg, bn, ST(t, l), ST(t, l) + F, nullptr, t->stat, t->grad);
+        RZ_LAUNCH_CHECK();
+        RZ_TRY(release(l, bn.off + bn.kf + 3 * (size_t)bn.C, 2 * (size_t)bn.C));
+        return partial_each([&](int, rz_trainer* p, int M, cudaStream_t s) {
+            bn_apply_kernel<<<grid_for((size_t)M * C), 256, 0, s>>>(yp(p), res(p), ld, C, M, p->blob, bn, ST(p, l), ST(p, l) + F, out(p));
+        });
+    };
+    // BN + ReLU backward of layer slot l (bn_backward)
+    auto bn_backward_g = [&](auto gp, auto ap, auto yp, int ld, int C, BnRef bn, int l, auto dyp, auto dz_out) -> int {
+        RZ_TRY(partial_each([&](int, rz_trainer* p, int M, cudaStream_t s) {
+            colred_partial_kernel<kBnGrad><<<chunks_of(M), 256, 0, s>>>(yp(p), ap(p), gp(p), ld, 0, C, M, ST(p, l), ST(p, l) + F, p->part);
+        }));
+        RZ_TRY(gather_part(2 * (size_t)C));
+        colred_finalize_kernel<kBnGrad><<<1, 256, 0, st>>>(t->part, chunks, C, Mg, bn, ST(t, l), ST(t, l) + F, ST(t, l) + 2 * F, t->stat,
+                                                           t->grad);
+        RZ_LAUNCH_CHECK();
+        RZ_TRY(release(l, 0, 0));
+        return partial_each([&](int, rz_trainer* p, int M, cudaStream_t s) {
+            bn_backward_kernel<<<grid_for((size_t)M * C), 256, 0, s>>>(gp(p), ap(p), yp(p), ld, C, M, Mg, p->blob, bn, ST(p, l), ST(p, l) + F,
+                                                                     ST(p, l) + 2 * F, dyp(p), dz_out(p));
+        });
+    };
+    auto none = [](rz_trainer*) { return (float*)nullptr; };
+    // split partials of layer l's weight gradient: the primary writes into its slot, a replica into its wpart and on
+    auto wgrad_g = [&](int l, int r, const float* in, int cin, const float* dyp, int rows, int z0, int nz, int per_l) -> int {
+        if (!nz) return RZ_OK;
+        rz_trainer* p = t->reps[r];
+        const size_t slice = (size_t)9 * cin * F;
+        float* dst = t->wgather + (size_t)l * t->wslot + (size_t)z0 * slice;
+        dim3 grid((9 * cin + kBM - 1) / kBM, (F + kBN - 1) / kBN, nz);
+        conv_gemm_tf32_kernel<true><<<grid, 256, 0, S(r)>>>(in, cin, dyp, F, nullptr, nullptr, r ? p->wpart : dst, rows * 64, per_l * 64);
+        RZ_LAUNCH_CHECK();
+        if (r) RZ_CUDA_TRY(peer(dst, 0, p->wpart, r, (size_t)nz * slice * sizeof(float), S(r)));
+        return RZ_OK;
+    };
+
+    // forward
+    for (int l = 0; l < L; ++l) {
+        RZ_TRY(partial_each([&](int, rz_trainer* p, int M, cudaStream_t s) {
+            const float* in = l ? A(p, l - 1) : p->x0;
+            const float* w = l ? p->blob + t->conv_off[l] : p->w0p;
+            return launch_conv(in, l ? F : kCin0, w, F, p->blob + t->conv_off[l] + bnref(l).kf, nullptr, Y(p, l), M, s);
+        }));
+        RZ_TRY(bn_forward_g([&](rz_trainer* p) { return Y(p, l); },
+                            [&](rz_trainer* p) { return (l >= 2 && l % 2 == 0) ? A(p, l - 2) : nullptr; }, F, F, bnref(l), l,
+                            [&](rz_trainer* p) { return A(p, l); }));
+    }
+    RZ_TRY(partial_each([&](int, rz_trainer* p, int M, cudaStream_t s) {
+        head_conv_kernel<<<(M * 32 + 255) / 256, 256, 0, s>>>(A(p, L - 1), F, M, p->blob, t->off_pc, t->off_vc, p->hc);
+    }));
+    const BnRef bpc{t->off_pc, (size_t)F * 2, 2}, bvc{t->off_vc, (size_t)F, 1};
+    RZ_TRY(bn_forward_g([](rz_trainer* p) { return p->hc; }, none, 3, 2, bpc, L, [](rz_trainer* p) { return p->ah; }));
+    RZ_TRY(bn_forward_g([](rz_trainer* p) { return p->hc + 2; }, none, 3, 1, bvc, L + 1, [](rz_trainer* p) { return p->ah + 2; }));
+
+    // loss and head backward; the per-record head tensors go to the primary
+    const size_t fc_smem = head_fc_smem(V);
+    RZ_TRY(partial_each([&](int, rz_trainer* p, int M, cudaStream_t s) {
+        head_fc_kernel<<<M / 64, 256, fc_smem, s>>>(p->ah, p->blob, t->ho, V, p->spol, p->sz, p->iota, p->act, batch, p->hp, p->hv, p->dl,
+                                                    p->h1, p->dh1, p->dv, p->lp, p->lv, p->dh);
+    }));
+    for (int r = 1; r < n; ++r) {
+        RZ_CUDA_TRY(on(r));
+        RZ_CUDA_TRY(cudaEventRecord(t->reps[r]->ev, S(r)));
+    }
+    RZ_CUDA_TRY(on(0));
+    for (int r = 1; r < n; ++r) {
+        if (!nr(r)) continue;
+        rz_trainer* p = t->reps[r];
+        RZ_CUDA_TRY(cudaStreamWaitEvent(st, p->ev, 0));
+        const size_t o = b0(r), k = nr(r), fb = sizeof(float);
+        RZ_CUDA_TRY(peer(t->hp + o * 128, 0, p->hp, r, k * 128 * fb, st));
+        RZ_CUDA_TRY(peer(t->hv + o * 64, 0, p->hv, r, k * 64 * fb, st));
+        RZ_CUDA_TRY(peer(t->dl + o * 64, 0, p->dl, r, k * 64 * fb, st));
+        RZ_CUDA_TRY(peer(t->h1 + o * V, 0, p->h1, r, k * V * fb, st));
+        RZ_CUDA_TRY(peer(t->dh1 + o * V, 0, p->dh1, r, k * V * fb, st));
+        RZ_CUDA_TRY(peer(t->dv + o, 0, p->dv, r, k * fb, st));
+        RZ_CUDA_TRY(peer(t->lp + o, 0, p->lp, r, k * fb, st));
+        RZ_CUDA_TRY(peer(t->lv + o, 0, p->lv, r, k * fb, st));
+    }
+    const int n_fc = 128 * 64 + 64 + 64 * V + 2 * V + 2;
+    head_fc_grad_kernel<<<(n_fc + 255) / 256, 256, 0, st>>>(t->hp, t->hv, t->dl, t->h1, t->dh1, t->dv, t->lp, t->lv, V, batch, t->ho,
+                                                            t->grad, t->loss_pv);
+    RZ_LAUNCH_CHECK();
+    RZ_TRY(bn_backward_g([](rz_trainer* p) { return p->dh; }, [](rz_trainer* p) { return p->ah; }, [](rz_trainer* p) { return p->hc; },
+                         3, 2, bpc, L, [](rz_trainer* p) { return p->dyh; }, none));
+    RZ_TRY(bn_backward_g([](rz_trainer* p) { return p->dh + 2; }, [](rz_trainer* p) { return p->ah + 2; },
+                         [](rz_trainer* p) { return p->hc + 2; }, 3, 1, bvc, L + 1, [](rz_trainer* p) { return p->dyh + 2; }, none));
+    RZ_TRY(partial_each([&](int, rz_trainer* p, int M, cudaStream_t s) {
+        colred_partial_kernel<kHeadConvGrad><<<chunks_of(M), 256, 0, s>>>(A(p, L - 1), nullptr, p->dyh, F, 3, F, M, nullptr, nullptr, p->part);
+    }));
+    RZ_TRY(gather_part(3 * (size_t)F));
+    colred_finalize_kernel<kHeadConvGrad><<<(F + 255) / 256, 256, 0, st>>>(t->part, chunks, F, Mg, BnRef{t->off_pc, t->off_vc, F}, nullptr,
+                                                                           nullptr, nullptr, t->stat, t->grad);
+    RZ_LAUNCH_CHECK();
+    RZ_TRY(release(-1, 0, 0));
+    RZ_TRY(partial_each([&](int, rz_trainer* p, int M, cudaStream_t s) {
+        head_conv_dgrad_kernel<<<grid_for((size_t)M * F), 256, 0, s>>>(p->dyh, p->blob, t->off_pc, t->off_vc, F, M, p->g);
+    }));
+
+    // tower backward
+    auto tower_wgrad = [&](int l, auto in) -> int {
+        for (int r = 0; r < n; ++r) {
+            if (!nr(r)) continue;
+            RZ_CUDA_TRY(on(r));
+            rz_trainer* p = t->reps[r];
+            RZ_TRY(wgrad_g(l, r, in(p), F, p->dy, nr(r), b0(r) / per, (nr(r) + per - 1) / per, per));
+        }
+        return RZ_OK;
+    };
+    auto dgrad = [&](int l, auto add, auto out) {
+        return partial_each([&](int, rz_trainer* p, int M, cudaStream_t s) {
+            return launch_conv(p->dy, F, p->wt + (size_t)(l - 1) * 9 * F * F, F, nullptr, add(p), out(p), M, s);
+        });
+    };
+    for (int i = R - 1; i >= 0; --i) {
+        const int l1 = 1 + 2 * i, l2 = l1 + 1;
+        RZ_TRY(bn_backward_g([](rz_trainer* p) { return p->g; }, [&](rz_trainer* p) { return A(p, l2); }, [&](rz_trainer* p) { return Y(p, l2); },
+                             F, F, bnref(l2), l2, [](rz_trainer* p) { return p->dy; }, [](rz_trainer* p) { return p->dz; }));
+        RZ_TRY(tower_wgrad(l2, [&](rz_trainer* p) { return A(p, l1); }));
+        RZ_TRY(dgrad(l2, none, [](rz_trainer* p) { return p->g1; }));
+        RZ_TRY(bn_backward_g([](rz_trainer* p) { return p->g1; }, [&](rz_trainer* p) { return A(p, l1); }, [&](rz_trainer* p) { return Y(p, l1); },
+                             F, F, bnref(l1), l1, [](rz_trainer* p) { return p->dy; }, none));
+        RZ_TRY(tower_wgrad(l1, [&](rz_trainer* p) { return A(p, l1 - 1); }));
+        RZ_TRY(dgrad(l1, [](rz_trainer* p) { return p->dz; }, [](rz_trainer* p) { return p->g; }));
+    }
+    RZ_TRY(bn_backward_g([](rz_trainer* p) { return p->g; }, [&](rz_trainer* p) { return A(p, 0); }, [&](rz_trainer* p) { return Y(p, 0); },
+                         F, F, bnref(0), 0, [](rz_trainer* p) { return p->dy; }, none));
+    // conv0: a split that straddles the end of shard r takes the first rows of layer 0's dy from replica r + 1 (the x0
+    // rows came with the staged records)
+    Conv0Share c0[64];
+    for (int r = 0; r < n; ++r) c0[r] = conv0_share(F, batch, b0(r), nr(r));
+    for (int r = 1; r < n; ++r) {
+        RZ_CUDA_TRY(on(r));
+        const int ov = c0[r - 1].ov;
+        if (ov) RZ_CUDA_TRY(peer(t->reps[r - 1]->dy + (size_t)nr(r - 1) * 64 * F, r - 1, t->reps[r]->dy, r, (size_t)ov * 64 * F * sizeof(float),
+                                 S(r)));
+        RZ_CUDA_TRY(cudaEventRecord(t->reps[r]->ev, S(r)));
+    }
+    for (int r = 0; r < n; ++r) {
+        if (!c0[r].nz) continue;
+        RZ_CUDA_TRY(on(r));
+        rz_trainer* p = t->reps[r];
+        if (c0[r].ov) RZ_CUDA_TRY(cudaStreamWaitEvent(S(r), t->reps[r + 1]->ev, 0));
+        RZ_TRY(wgrad_g(0, r, p->x0 + (size_t)c0[r].row0 * 64 * kCin0, kCin0, p->dy + (size_t)c0[r].row0 * 64 * F, c0[r].rows, c0[r].z0,
+                       c0[r].nz, per0));
+    }
+
+    // join the replicas' partials, reduce every layer in split order, hand the gradient out, update everywhere
+    for (int r = 1; r < n; ++r) {
+        RZ_CUDA_TRY(on(r));
+        RZ_CUDA_TRY(cudaEventRecord(t->reps[r]->ev, S(r)));
+    }
+    RZ_CUDA_TRY(on(0));
+    for (int r = 1; r < n; ++r) RZ_CUDA_TRY(cudaStreamWaitEvent(st, t->reps[r]->ev, 0));
+    for (int l = 0; l < L; ++l) {
+        const int cin = l ? F : kCin0, pl = l ? per : per0;
+        wgrad_reduce_kernel<<<grid_for((size_t)9 * cin * F), 256, 0, st>>>(t->wgather + (size_t)l * t->wslot, (batch + pl - 1) / pl, cin,
+                                                                           l ? F : 2, F, t->grad + t->conv_off[l]);
+    }
+    RZ_LAUNCH_CHECK();
+    RZ_CUDA_TRY(cudaEventRecord(t->ev, st));
+    for (int r = 1; r < n; ++r) {
+        rz_trainer* p = t->reps[r];
+        RZ_CUDA_TRY(on(r));
+        RZ_CUDA_TRY(cudaStreamWaitEvent(p->stream, t->ev, 0));
+        RZ_CUDA_TRY(peer(p->grad, r, t->grad, 0, t->n * sizeof(float), p->stream));
+        RZ_CUDA_TRY(peer(p->bad, r, t->bad, 0, sizeof(int), p->stream));
+        update_kernel<<<kUpdateBlocks, 256, 0, p->stream>>>(p->blob, p->vel, p->grad, p->stat, p->kind, t->n, lr, t->cfg.momentum,
+                                                            t->cfg.l2_reg, t->cfg.bn_momentum, p->bad, p->l2_part);
+        RZ_LAUNCH_CHECK();
+        RZ_CUDA_TRY(cudaEventRecord(p->ev, p->stream));
+    }
+    RZ_CUDA_TRY(on(0));
+    for (int r = 1; r < n; ++r) RZ_CUDA_TRY(cudaStreamWaitEvent(st, t->reps[r]->ev, 0));  // update_kernel rewrites grad
+    update_kernel<<<kUpdateBlocks, 256, 0, st>>>(t->blob, t->vel, t->grad, t->stat, t->kind, t->n, lr, t->cfg.momentum, t->cfg.l2_reg,
+                                                  t->cfg.bn_momentum, t->bad, t->l2_part);
+    loss_kernel<<<1, 32, 0, st>>>(t->l2_part, t->loss_pv, t->cfg.l2_reg, t->bad, loss);
+    RZ_LAUNCH_CHECK();
+    return RZ_OK;
+}
+
+int check_cfg(const rz_net_cfg* net, const rz_train_cfg* cfg) {
     RZ_REQUIRE(net->kernel_size == 3, "trainer: only cnn_filter_size == 3 is supported (got %d)", net->kernel_size);
     RZ_REQUIRE(net->filters >= 16 && net->filters <= 256 && net->filters % 16 == 0,
                "trainer: cnn_filter_num must be a multiple of 16 in [16, 256] (got %d)", net->filters);
@@ -788,12 +1152,20 @@ int rz_trainer_create(const rz_net_cfg* net, const rz_train_cfg* cfg, int device
                "trainer: unsupported model configuration (res_blocks=%d value_fc=%d)", net->res_blocks, net->value_fc);
     RZ_REQUIRE(cfg->max_batch >= 1 && cfg->max_batch <= 65536, "trainer: max_batch must be in [1, 65536] (got %d)", cfg->max_batch);
     RZ_REQUIRE(isfinite(cfg->momentum) && isfinite(cfg->l2_reg) && isfinite(cfg->bn_momentum), "trainer: non-finite setting");
+    return RZ_OK;
+}
+
+// A trainer, or one replica of a group: activation and backward buffers for `act` records, the batch-wide buffers (column
+// partials, per-record head tensors, staged records) for `full`.  A single trainer has act = full = max_batch.
+int trainer_create(const rz_net_cfg* net, const rz_train_cfg* cfg, int device, size_t act, size_t full, bool group, bool primary,
+                   rz_trainer** out) {
     RZ_CUDA_TRY(cudaSetDevice(device));
     rz_trainer* t = new (std::nothrow) rz_trainer();
     if (!t) { set_error("out of host memory"); return RZ_ENOMEM; }
     t->net = *net;
     t->cfg = *cfg;
     t->device = device;
+    t->act = act;
     const int F = net->filters, R = net->res_blocks, V = net->value_fc;
     t->F = F; t->R = R; t->V = V; t->L = 1 + 2 * R;
     // blob layout of rz_net_load_weights (include/rz_engine.h), with the kind of every entry
@@ -818,9 +1190,9 @@ int rz_trainer_create(const rz_net_cfg* net, const rz_train_cfg* cfg, int device
     t->ho.v2b = kind.size(); kind.insert(kind.end(), 1, kTrainable);
     t->n = kind.size();
 
-    const size_t B = cfg->max_batch, M = 64 * B, MF = M * F, L = t->L;
-    t->wgrad_splits_max = wgrad_splits(F, F, (int)B);
-    const int s0 = wgrad_splits(kCin0, F, (int)B);
+    const size_t B = full, M = 64 * act, MF = M * F, L = t->L;
+    t->wgrad_splits_max = wgrad_splits(F, F, cfg->max_batch);
+    const int s0 = wgrad_splits(kCin0, F, cfg->max_batch);
     const size_t wpart = std::max((size_t)t->wgrad_splits_max * 9 * F * F, (size_t)s0 * 9 * kCin0 * F);
     struct { float** p; size_t n; } allocs[] = {
         {&t->blob, t->n}, {&t->vel, t->n}, {&t->grad, t->n}, {&t->stat, t->n}, {&t->x0, M * kCin0}, {&t->w0p, (size_t)9 * kCin0 * F},
@@ -831,6 +1203,19 @@ int rz_trainer_create(const rz_net_cfg* net, const rz_train_cfg* cfg, int device
     cudaError_t e = cudaSuccess;
     for (auto& a : allocs)
         if (e == cudaSuccess) e = cudaMalloc(a.p, a.n * sizeof(float));
+    if (group) {
+        t->wslot = wpart;
+        std::vector<int32_t> iota(act);
+        for (size_t i = 0; i < act; ++i) iota[i] = (int32_t)i;
+        if (e == cudaSuccess) e = cudaMalloc(&t->sp, B * 128);
+        if (e == cudaSuccess) e = cudaMalloc(&t->spol, B * 64 * sizeof(float));
+        if (e == cudaSuccess) e = cudaMalloc(&t->sz, B * sizeof(float));
+        if (e == cudaSuccess) e = cudaMalloc(&t->iota, act * sizeof(int32_t));
+        if (e == cudaSuccess) e = cudaMemcpy(t->iota, iota.data(), act * sizeof(int32_t), cudaMemcpyHostToDevice);
+        if (e == cudaSuccess && primary) e = cudaMalloc(&t->wgather, L * wpart * sizeof(float));
+        if (e == cudaSuccess && !primary) e = cudaStreamCreateWithFlags(&t->stream, cudaStreamNonBlocking);
+        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&t->ev, cudaEventDisableTiming);
+    }
     if (e == cudaSuccess) e = cudaMalloc(&t->part, B * 3 * F * sizeof(double));
     if (e == cudaSuccess) e = cudaMalloc(&t->kind, t->n);
     if (e == cudaSuccess) e = cudaMalloc(&t->bad, sizeof(int));
@@ -852,11 +1237,74 @@ int rz_trainer_create(const rz_net_cfg* net, const rz_train_cfg* cfg, int device
     return RZ_OK;
 }
 
-int rz_trainer_destroy(rz_trainer* t) {
-    if (!t) return RZ_OK;
+void trainer_delete(rz_trainer* t) {
+    for (size_t r = 1; r < t->reps.size(); ++r) trainer_delete(t->reps[r]);
     cudaSetDevice(t->device);
     trainer_free(t);
     delete t;
+}
+
+}  // namespace
+
+extern "C" {
+
+int rz_train_shard_plan_host(int filters, int res_blocks, int batch, int n_devices, int32_t* bounds) {
+    RZ_REQUIRE(bounds, "rz_train_shard_plan_host: null pointer");
+    RZ_REQUIRE(filters >= 16 && filters <= 256 && filters % 16 == 0 && res_blocks >= 0 && batch >= 1 && n_devices >= 1 && n_devices <= 64,
+               "rz_train_shard_plan_host: bad arguments");
+    int b[65];
+    shard_plan(filters, res_blocks, batch, n_devices, b);
+    for (int r = 0; r <= n_devices; ++r) bounds[r] = b[r];
+    return RZ_OK;
+}
+
+int rz_trainer_create(const rz_net_cfg* net, const rz_train_cfg* cfg, int device, rz_trainer** out) {
+    RZ_REQUIRE(net && cfg && out, "rz_trainer_create: null pointer");
+    RZ_TRY(check_cfg(net, cfg));
+    return trainer_create(net, cfg, device, cfg->max_batch, cfg->max_batch, false, true, out);
+}
+
+int rz_trainer_create_group(const rz_net_cfg* net, const rz_train_cfg* cfg, const int* devices, int n_devices, rz_trainer** out) {
+    RZ_REQUIRE(net && cfg && devices && out, "rz_trainer_create_group: null pointer");
+    RZ_REQUIRE(n_devices >= 1 && n_devices <= 64, "rz_trainer_create_group: n_devices must be in [1, 64] (got %d)", n_devices);
+    int count = 0;
+    RZ_CUDA_TRY(cudaGetDeviceCount(&count));
+    for (int r = 0; r < n_devices; ++r)
+        RZ_REQUIRE(devices[r] >= 0 && devices[r] < count, "rz_trainer_create_group: device %d is not one of the %d visible devices",
+                   devices[r], count);
+    if (n_devices == 1) return rz_trainer_create(net, cfg, devices[0], out);
+    RZ_TRY(check_cfg(net, cfg));
+    // each replica's largest shard over every batch it can be given, with the records of conv0's straddling split
+    std::vector<size_t> act(n_devices, 1);
+    int b[65];
+    for (int batch = 1; batch <= cfg->max_batch; ++batch) {
+        shard_plan(net->filters, net->res_blocks, batch, n_devices, b);
+        for (int r = 0; r < n_devices; ++r) {
+            const int len = b[r + 1] - b[r], ov = conv0_share(net->filters, batch, b[r], len).ov;
+            act[r] = std::max(act[r], (size_t)(len + ov));
+        }
+    }
+    rz_trainer* t = nullptr;
+    RZ_TRY(trainer_create(net, cfg, devices[0], act[0], cfg->max_batch, true, true, &t));
+    t->reps.push_back(t);
+    for (int r = 1; r < n_devices; ++r) {
+        rz_trainer* p = nullptr;
+        const int rc = trainer_create(net, cfg, devices[r], act[r], act[r], true, false, &p);
+        if (rc != RZ_OK) {
+            trainer_delete(t);
+            cudaSetDevice(devices[0]);
+            return rc;
+        }
+        t->reps.push_back(p);
+    }
+    RZ_CUDA_TRY(cudaSetDevice(devices[0]));
+    *out = t;
+    return RZ_OK;
+}
+
+int rz_trainer_destroy(rz_trainer* t) {
+    if (!t) return RZ_OK;
+    trainer_delete(t);
     return RZ_OK;
 }
 
@@ -869,9 +1317,12 @@ int rz_trainer_blob_size(const rz_trainer* t, size_t* n_floats) {
 int rz_trainer_load_weights(rz_trainer* t, const float* blob_host, size_t n_floats) {
     RZ_REQUIRE(t && blob_host, "rz_trainer_load_weights: null pointer");
     RZ_REQUIRE(n_floats == t->n, "weight blob has %zu floats, this configuration needs %zu", n_floats, t->n);
+    for (rz_trainer* p : t->reps.empty() ? std::vector<rz_trainer*>{t} : t->reps) {
+        RZ_CUDA_TRY(cudaSetDevice(p->device));
+        RZ_CUDA_TRY(cudaMemcpy(p->blob, blob_host, n_floats * sizeof(float), cudaMemcpyHostToDevice));
+        RZ_CUDA_TRY(cudaMemset(p->vel, 0, n_floats * sizeof(float)));
+    }
     RZ_CUDA_TRY(cudaSetDevice(t->device));
-    RZ_CUDA_TRY(cudaMemcpy(t->blob, blob_host, n_floats * sizeof(float), cudaMemcpyHostToDevice));
-    RZ_CUDA_TRY(cudaMemset(t->vel, 0, n_floats * sizeof(float)));
     t->loaded = true;
     return RZ_OK;
 }
@@ -882,6 +1333,11 @@ int rz_trainer_load_weights_dev(rz_trainer* t, const float* blob_dev, size_t n_f
     RZ_CUDA_TRY(cudaSetDevice(t->device));
     RZ_CUDA_TRY(cudaMemcpyAsync(t->blob, blob_dev, n_floats * sizeof(float), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
     RZ_CUDA_TRY(cudaMemsetAsync(t->vel, 0, n_floats * sizeof(float), (cudaStream_t)stream));
+    for (size_t r = 1; r < t->reps.size(); ++r) {  // the replicas copy the primary, in the caller's stream order
+        rz_trainer* p = t->reps[r];
+        RZ_CUDA_TRY(cudaMemcpyPeerAsync(p->blob, p->device, t->blob, t->device, n_floats * sizeof(float), (cudaStream_t)stream));
+        RZ_CUDA_TRY(cudaMemcpyPeerAsync(p->vel, p->device, t->vel, t->device, n_floats * sizeof(float), (cudaStream_t)stream));
+    }
     t->loaded = true;
     return RZ_OK;
 }
@@ -903,7 +1359,22 @@ int rz_trainer_step_dev(rz_trainer* t, const uint8_t* planes, const float* polic
     RZ_REQUIRE(isfinite(lr), "rz_trainer_step_dev: non-finite learning rate");
     if (!t->loaded) { set_error("rz_trainer: weights not loaded"); return RZ_ESTATE; }
     RZ_CUDA_TRY(cudaSetDevice(t->device));
-    return trainer_step(t, planes, policy, z, index, n_records, (int)batch, lr, loss_dev, (cudaStream_t)stream);
+    if (t->reps.empty()) return trainer_step(t, planes, policy, z, index, n_records, (int)batch, lr, loss_dev, (cudaStream_t)stream);
+    const int rc = group_step(t, planes, policy, z, index, n_records, (int)batch, lr, loss_dev, (cudaStream_t)stream);
+    cudaSetDevice(t->device);
+    return rc;
+}
+
+int rz_trainer_replica_state_dev(rz_trainer* t, int r, float* blob_dev, float* vel_dev, size_t n_floats, void* stream) {
+    RZ_REQUIRE(t && blob_dev && vel_dev, "rz_trainer_replica_state_dev: null pointer");
+    RZ_REQUIRE(n_floats == t->n, "weight blob has %zu floats, this configuration needs %zu", n_floats, t->n);
+    const int n = t->reps.empty() ? 1 : (int)t->reps.size();
+    RZ_REQUIRE(r >= 0 && r < n, "rz_trainer_replica_state_dev: replica %d outside [0, %d)", r, n);
+    const rz_trainer* p = r ? t->reps[r] : t;
+    RZ_CUDA_TRY(cudaSetDevice(t->device));
+    RZ_CUDA_TRY(cudaMemcpyPeerAsync(blob_dev, t->device, p->blob, p->device, n_floats * sizeof(float), (cudaStream_t)stream));
+    RZ_CUDA_TRY(cudaMemcpyPeerAsync(vel_dev, t->device, p->vel, p->device, n_floats * sizeof(float), (cudaStream_t)stream));
+    return RZ_OK;
 }
 
 int rz_trainer_last_grad_dev(rz_trainer* t, float* grad_dev, size_t n_floats, void* stream) {

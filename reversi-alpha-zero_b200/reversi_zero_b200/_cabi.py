@@ -118,6 +118,8 @@ SIGNATURES = {
     "rz_ingest_json_host": (C.c_int, [vp, sz, sz, vp, vp, vp, C.POINTER(sz), C.POINTER(sz)]),
     "rz_ingest_json": (C.c_int, [C.c_char_p, sz, vp, vp, vp, C.POINTER(sz), C.POINTER(sz)]),
     "rz_trainer_create": (C.c_int, [C.POINTER(NetCfg), C.POINTER(TrainCfg), C.c_int, C.POINTER(vp)]),
+    "rz_trainer_create_group": (C.c_int, [C.POINTER(NetCfg), C.POINTER(TrainCfg), i32p, C.c_int, C.POINTER(vp)]),
+    "rz_train_shard_plan_host": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, i32p]),
     "rz_trainer_destroy": (C.c_int, [vp]),
     "rz_trainer_blob_size": (C.c_int, [vp, C.POINTER(sz)]),
     "rz_trainer_load_weights": (C.c_int, [vp, f32p, sz]),
@@ -125,6 +127,7 @@ SIGNATURES = {
     "rz_trainer_weights_dev": (C.c_int, [vp, vp, sz, vp]),
     "rz_trainer_step_dev": (C.c_int, [vp, vp, vp, vp, sz, vp, sz, C.c_float, vp, vp]),
     "rz_trainer_last_grad_dev": (C.c_int, [vp, vp, sz, vp]),
+    "rz_trainer_replica_state_dev": (C.c_int, [vp, C.c_int, vp, vp, sz, vp]),
     "rz_trainer_debug_conv_dev": (C.c_int, [vp, C.c_int, vp, vp, vp, vp, sz, vp, vp]),
 }
 

@@ -6,6 +6,10 @@ on a device-resident dataset (what ``worker.ingest.to_training_tensors`` returns
     tr.load_blob(blob)
     loss = tr.step(states, policy, z, index, lr)   # index: int32 CUDA tensor of record numbers (a slice of a permutation)
     net.load_blob_dev(tr.blob_dev())
+
+``Trainer(model_config, max_batch, devices=[0, 1, 2, 3])`` trains one batch across several devices (a data-parallel
+group, rz_trainer_create_group): the same calls, the dataset and index on ``devices[0]``, and exactly the bits of the
+one-device step.
 """
 import ctypes as C
 
@@ -21,16 +25,29 @@ CONV0_FWD, CONV_FWD, CONV_DGRAD, CONV_WGRAD, CONV0_WGRAD = 0, 1, 2, 3, 4
 
 
 class Trainer:
-    def __init__(self, model_config, max_batch, device=0, momentum=MOMENTUM, bn_momentum=BN_MOMENTUM, l2_reg=None):
+    def __init__(self, model_config, max_batch, device=0, devices=None, momentum=MOMENTUM, bn_momentum=BN_MOMENTUM, l2_reg=None):
+        """``devices``: a list of CUDA ordinals (repeats allowed) builds a data-parallel group whose primary is
+        ``devices[0]``; ``device`` is then ignored.  None trains on ``device`` alone."""
         import torch
+        if devices is not None:
+            devices = list(devices)
+            if not all(isinstance(d, (int, np.integer)) and not isinstance(d, bool) for d in devices):
+                raise TypeError(f"devices must be a list of CUDA ordinals, got {devices!r}")
+            devices = [int(d) for d in devices]
         self.mc = model_config
-        self.device = torch.device("cuda", device)
+        self.devices = devices
         self.max_batch = int(max_batch)
         self._h = C.c_void_p()
         ncfg = _cabi.NetCfg(model_config.cnn_filter_num, model_config.res_layer_num, model_config.value_fc_size,
                             model_config.cnn_filter_size)
         tcfg = _cabi.TrainCfg(self.max_batch, momentum, model_config.l2_reg if l2_reg is None else l2_reg, bn_momentum)
-        _cabi.check(_cabi.lib().rz_trainer_create(C.byref(ncfg), C.byref(tcfg), device, C.byref(self._h)), "rz_trainer_create")
+        if devices is None:
+            _cabi.check(_cabi.lib().rz_trainer_create(C.byref(ncfg), C.byref(tcfg), device, C.byref(self._h)), "rz_trainer_create")
+        else:
+            ords = (C.c_int32 * max(len(devices), 1))(*devices)
+            _cabi.check(_cabi.lib().rz_trainer_create_group(C.byref(ncfg), C.byref(tcfg), ords, len(devices), C.byref(self._h)),
+                        "rz_trainer_create_group")
+        self.device = torch.device("cuda", devices[0] if devices else device)
         n = C.c_size_t()
         _cabi.check(_cabi.lib().rz_trainer_blob_size(self._h, C.byref(n)), "rz_trainer_blob_size")
         self.blob_floats = n.value
@@ -86,6 +103,15 @@ class Trainer:
         _cabi.check(_cabi.lib().rz_trainer_last_grad_dev(self._h, C.c_void_p(out.data_ptr()), out.numel(), self._stream()),
                     "rz_trainer_last_grad_dev")
         return out.cpu().numpy()
+
+    def replica_state(self, r):
+        """test hook: (weights, momentum) of replica ``r`` (0 = the primary) as float32 CUDA tensors on the primary"""
+        import torch
+        w = torch.empty(self.blob_floats, dtype=torch.float32, device=self.device)
+        v = torch.empty_like(w)
+        _cabi.check(_cabi.lib().rz_trainer_replica_state_dev(self._h, r, C.c_void_p(w.data_ptr()), C.c_void_p(v.data_ptr()), w.numel(),
+                                                             self._stream()), "rz_trainer_replica_state_dev")
+        return w, v
 
     def debug_conv(self, op, x, batch, kernel=None, bias=None, add=None):
         """test hook (rz_trainer_debug_conv_dev): one of the step's convolution GEMMs, CONV_* below, on float32 CUDA

@@ -16,7 +16,9 @@ Differences, all on the data path:
     numpy's global RNG);
   * a model is saved as ``next_generation/model_<ts>/model_weight.rzblob.npy`` only, built in a directory whose name does
     not match ``model_*`` and renamed into place, so self-play's reload and the evaluator never see a half-written model;
-  * momentum lives in device memory only (the reference does not persist it either).
+  * momentum lives in device memory only (the reference does not persist it either);
+  * with ``b200.train_devices`` (a list of CUDA ordinals) each batch is trained across those devices by one data-parallel
+    trainer, bit for bit as on one device; the dataset lives on the first of them.
 """
 import os
 import time
@@ -81,16 +83,20 @@ class PerStepCallback:
 
 class OptimizeWorker:
     def __init__(self, config, device=0, trainer=None, to_tensors=None, sleep=time.sleep, clock=time.time, seed=0,
-                 read_json=None):
-        """``trainer`` (an object with load_blob / step / blob, default ``train.Trainer``), ``to_tensors`` (rows ->
+                 read_json=None, trainer_cls=None):
+        """``trainer`` (an object with load_blob / step / blob, default ``trainer_cls(model_config, max_batch=...,
+        device=..., devices=b200.train_devices)`` with ``trainer_cls`` = ``train.Trainer``), ``to_tensors`` (rows ->
         (states, policy, z) tensors, default ``ingest.to_training_tensors`` on ``device``) and ``read_json`` (a
         play_*.json path -> the same tensors, default ``ingest.read_play_json`` on ``device``) can be replaced, e.g. by
         stand-ins in host-only tests."""
         self.config = config
-        self.device = device
+        # a data-parallel trainer's dataset lives on its primary, devices[0]
+        self.train_devices = getattr(getattr(config, "b200", None), "train_devices", None)
+        self.device = self.train_devices[0] if self.train_devices else device
         self.trainer = trainer
-        self.to_tensors = to_tensors or (lambda rows, tau1, ctt: ingest.to_training_tensors(rows, tau1, ctt, device))
-        self.read_json = read_json or (lambda path: ingest.read_play_json(path, device))
+        self.trainer_cls = trainer_cls
+        self.to_tensors = to_tensors or (lambda rows, tau1, ctt: ingest.to_training_tensors(rows, tau1, ctt, self.device))
+        self.read_json = read_json or (lambda path: ingest.read_play_json(path, self.device))
         # the source of the training data: JSON can come from writers whose config this process cannot see
         self.train_from_json = bool(getattr(getattr(config, "b200", None), "train_from_json", False))
         self.sleep, self.clock = sleep, clock
@@ -184,7 +190,8 @@ class OptimizeWorker:
                 raise RuntimeError(f"Best model can not loaded! ({path} does not exist)")
         if self.trainer is None:
             from ..train import Trainer
-            self.trainer = Trainer(self.config.model, max_batch=trainer_field(self.config, "batch_size"), device=self.device)
+            self.trainer = (self.trainer_cls or Trainer)(self.config.model, max_batch=trainer_field(self.config, "batch_size"),
+                                                         device=self.device, devices=self.train_devices)
         self.trainer.load_blob(np.load(path))
         logger.debug(f"loaded model from {path}")
         return path
