@@ -652,7 +652,6 @@ struct rz_trainer {
     size_t off_pc, off_vc;  // policy / value head conv kernels
     HeadOffs ho;
     std::vector<size_t> conv_off;  // kernel offset of tower convolution l
-    int wgrad_splits_max;
 
     float *blob, *vel, *grad, *stat;
     uint8_t* kind;
@@ -663,20 +662,21 @@ struct rz_trainer {
     float *hp, *hv, *dl, *h1, *dh1, *dv, *lp, *lv;  // per-record head tensors
     float *stats;                 // [L + 2][4][F]: mean, invstd, sum dz, sum dz*xhat
     double *part;                 // column-reduction partials [max_batch][3][F] ([act][3][F] on replicas 1..)
-    float *wpart;                 // weight-gradient split-K partials
+    float *wpart;                 // weight-gradient split-K partials [wslot]
+    size_t wslot;                 // floats of the split partials of the largest layer at max_batch
     float *l2_part, *loss_pv;
     int* bad;
     size_t act;                   // records the activation and backward buffers hold (max_batch for a single trainer)
 
-    // data-parallel group (rz_trainer_create_group): the handle is replica 0, the primary; a single trainer has none
+    // The handle is replica 0, the primary, of a data-parallel group (rz_trainer_create_group).  A single trainer is the
+    // group of that one replica and owns nothing below `reps`.
     std::vector<rz_trainer*> reps;  // every replica, reps[0] = this
     cudaStream_t stream;          // replicas 1..: the stream the trainer owns (the primary runs on the caller's stream)
     cudaEvent_t ev;               // marks this replica's progress at each exchange
     uint8_t* sp;                  // staged batch records: planes [.][128], policy [.][64], z [.] (primary: max_batch)
     float *spol, *sz;
-    int32_t* iota;                // identity index [act]: the staged records are the replica's dataset
+    int32_t* iota;                // replicas 1..: identity index [act]: the staged records are the replica's dataset
     float* wgather;               // primary: every layer's weight-gradient split partials [L][wslot], reduced after the join
-    size_t wslot;
 };
 
 namespace {
@@ -707,9 +707,9 @@ int wgrad_per(int cin, int F, int batch) {
     return (batch + splits - 1) / splits;
 }
 
-// Shards of a group step: replica r trains on records [bounds[r], bounds[r + 1]).  The boundaries sit on the weight-
-// gradient split grid of the F->F convolutions (conv0's grid without residual blocks), so every split of those layers
-// lies inside one shard; the grid's cells are dealt out as evenly as possible, the larger shares first.
+// Shards of a step: replica r trains on records [bounds[r], bounds[r + 1]).  The boundaries sit on the weight-gradient
+// split grid of the F->F convolutions (conv0's grid without residual blocks), so every split of those layers lies
+// inside one shard; the grid's cells are dealt out as evenly as possible, the larger shares first.
 void shard_plan(int F, int R, int batch, int n, int* bounds) {
     const int per = wgrad_per(R ? F : kCin0, F, batch), cells = (batch + per - 1) / per;
     const int q = cells / n, rem = cells % n;
@@ -740,113 +740,36 @@ int launch_conv(const float* in, int cin, const float* w, int F, const float* bi
     return RZ_OK;
 }
 
-// dw (blob layout [9][cin_real][F]) = weight gradient of a conv with input `in` [M][cin] and output gradient dy [M][F]
-int launch_wgrad(rz_trainer* t, const float* in, int cin, int cin_real, const float* dyp, int M, float* dw, cudaStream_t st) {
-    const int F = t->F, batch = M / 64, splits = wgrad_splits(cin, F, batch);
-    const int per = (batch + splits - 1) / splits, used = (batch + per - 1) / per;
-    dim3 grid((9 * cin + kBM - 1) / kBM, (F + kBN - 1) / kBN, used);
-    conv_gemm_tf32_kernel<true><<<grid, 256, 0, st>>>(in, cin, dyp, F, nullptr, nullptr, t->wpart, M, per * 64);
-    wgrad_reduce_kernel<<<grid_for((size_t)9 * cin * F), 256, 0, st>>>(t->wpart, used, cin, cin_real, F, dw);
+// `nz` consecutive split-K partials of a convolution's weight gradient into part[nz][9 * cin][F]: the k-th covers records
+// [k * per, (k + 1) * per) of the input `in` [rows * 64][cin] and of the output gradient dyp [rows * 64][F].  Given dw,
+// they are all of the layer's splits and are reduced at once into dw (blob layout [9][cin_real][F]).
+int launch_wgrad(const float* in, int cin, int cin_real, const float* dyp, int F, int rows, int nz, int per, float* part, float* dw,
+                 cudaStream_t st) {
+    dim3 grid((9 * cin + kBM - 1) / kBM, (F + kBN - 1) / kBN, nz);
+    conv_gemm_tf32_kernel<true><<<grid, 256, 0, st>>>(in, cin, dyp, F, nullptr, nullptr, part, rows * 64, per * 64);
+    if (dw) wgrad_reduce_kernel<<<grid_for((size_t)9 * cin * F), 256, 0, st>>>(part, nz, cin, cin_real, F, dw);
     RZ_LAUNCH_CHECK();
     return RZ_OK;
 }
 
-// training-mode BN forward of a [M][ld] tensor (channels [0, C)): statistics, then normalise (+ residual) + ReLU
-void bn_forward(rz_trainer* t, const float* yp, const float* res, int ld, int C, int M, BnRef bn, float* st4, float* out,
-                cudaStream_t st) {
-    const int chunks = (M + kRowsPerChunk - 1) / kRowsPerChunk;
-    float *mean = st4, *invstd = st4 + t->F;
-    colred_partial_kernel<kSum><<<chunks, 256, 0, st>>>(yp, nullptr, nullptr, ld, 0, C, M, nullptr, nullptr, t->part);
-    colred_finalize_kernel<kSum><<<1, 256, 0, st>>>(t->part, chunks, C, M, bn, mean, invstd, nullptr, t->stat, t->grad);
-    colred_partial_kernel<kSqDev><<<chunks, 256, 0, st>>>(yp, nullptr, nullptr, ld, 0, C, M, mean, nullptr, t->part);
-    colred_finalize_kernel<kSqDev><<<1, 256, 0, st>>>(t->part, chunks, C, M, bn, mean, invstd, nullptr, t->stat, t->grad);
-    bn_apply_kernel<<<grid_for((size_t)M * C), 256, 0, st>>>(yp, res, ld, C, M, t->blob, bn, mean, invstd, out);
-}
+// A tensor of the step that every replica holds, named once for all of them: p->*buf + layer * (p's layer stride) + col
+using TrainerBuf = float* rz_trainer::*;
+struct Operand {
+    TrainerBuf buf = nullptr;  // null: no operand
+    int layer = 0, col = 0;
+};
 
-// BN + ReLU backward: gp = gradient of the layer output; writes dyp (gradient of the conv output) and, when dz_out is
-// given, the gradient below the ReLU (what the skip connection carries); gamma / beta gradients into t->grad
-void bn_backward(rz_trainer* t, const float* gp, const float* ap, const float* yp, int ld, int C, int M, BnRef bn, float* st4,
-                 float* dyp, float* dz_out, cudaStream_t st) {
-    const int chunks = (M + kRowsPerChunk - 1) / kRowsPerChunk;
-    float *mean = st4, *invstd = st4 + t->F, *sums = st4 + 2 * t->F;
-    colred_partial_kernel<kBnGrad><<<chunks, 256, 0, st>>>(yp, ap, gp, ld, 0, C, M, mean, invstd, t->part);
-    colred_finalize_kernel<kBnGrad><<<1, 256, 0, st>>>(t->part, chunks, C, M, bn, mean, invstd, sums, t->stat, t->grad);
-    bn_backward_kernel<<<grid_for((size_t)M * C), 256, 0, st>>>(gp, ap, yp, ld, C, M, M, t->blob, bn, mean, invstd, sums, dyp, dz_out);
-}
+// The dataset a replica reads its shard from
+struct Records {
+    const uint8_t* planes;
+    const float *policy, *z;
+    const int32_t* index;
+    size_t n;
+};
 
-int trainer_step(rz_trainer* t, const uint8_t* planes, const float* policy, const float* z, const int32_t* index, size_t n_records,
-                 int batch, float lr, float* loss, cudaStream_t st) {
-    const int F = t->F, R = t->R, L = t->L, V = t->V, M = batch * 64;
-    const size_t MF = (size_t)M * F, lstride = (size_t)64 * t->act * F;
-    auto Y = [&](int l) { return t->y + (size_t)l * lstride; };
-    auto A = [&](int l) { return t->a + (size_t)l * lstride; };
-    auto ST = [&](int l) { return t->stats + (size_t)l * 4 * F; };
-    auto bnref = [&](int l) { return BnRef{t->conv_off[l], (size_t)9 * (l ? F : 2) * F, F}; };
-
-    RZ_CUDA_TRY(cudaMemsetAsync(t->bad, 0, sizeof(int), st));
-    gather_kernel<<<(M * kCin0 + 255) / 256, 256, 0, st>>>(planes, index, n_records, batch, t->x0, t->bad);
-    pack_w0_kernel<<<(9 * kCin0 * F + 255) / 256, 256, 0, st>>>(t->blob + t->conv_off[0], F, t->w0p);
-    for (int l = 1; l < L; ++l)
-        pack_wt_kernel<<<grid_for((size_t)9 * F * F), 256, 0, st>>>(t->blob + t->conv_off[l], F, t->wt + (size_t)(l - 1) * 9 * F * F);
-    RZ_LAUNCH_CHECK();
-
-    // forward
-    for (int l = 0; l < L; ++l) {
-        const float* in = l ? A(l - 1) : t->x0;
-        const float* w = l ? t->blob + t->conv_off[l] : t->w0p;
-        const float* bias = t->blob + t->conv_off[l] + bnref(l).kf;
-        RZ_TRY(launch_conv(in, l ? F : kCin0, w, F, bias, nullptr, Y(l), M, st));
-        const float* res = (l >= 2 && l % 2 == 0) ? A(l - 2) : nullptr;  // conv2 of a block adds the block input
-        bn_forward(t, Y(l), res, F, F, M, bnref(l), ST(l), A(l), st);
-    }
-    const float* tower = A(L - 1);
-    head_conv_kernel<<<(M * 32 + 255) / 256, 256, 0, st>>>(tower, F, M, t->blob, t->off_pc, t->off_vc, t->hc);
-    const BnRef bpc{t->off_pc, (size_t)F * 2, 2}, bvc{t->off_vc, (size_t)F, 1};
-    bn_forward(t, t->hc, nullptr, 3, 2, M, bpc, ST(L), t->ah, st);
-    bn_forward(t, t->hc + 2, nullptr, 3, 1, M, bvc, ST(L + 1), t->ah + 2, st);
-
-    // loss and head backward
-    const size_t fc_smem = head_fc_smem(V);
-    head_fc_kernel<<<batch, 256, fc_smem, st>>>(t->ah, t->blob, t->ho, V, policy, z, index, n_records, batch, t->hp, t->hv, t->dl,
-                                                t->h1, t->dh1, t->dv, t->lp, t->lv, t->dh);
-    const int n_fc = 128 * 64 + 64 + 64 * V + 2 * V + 2;
-    head_fc_grad_kernel<<<(n_fc + 255) / 256, 256, 0, st>>>(t->hp, t->hv, t->dl, t->h1, t->dh1, t->dv, t->lp, t->lv, V, batch, t->ho,
-                                                            t->grad, t->loss_pv);
-    RZ_LAUNCH_CHECK();
-    bn_backward(t, t->dh, t->ah, t->hc, 3, 2, M, bpc, ST(L), t->dyh, nullptr, st);
-    bn_backward(t, t->dh + 2, t->ah + 2, t->hc + 2, 3, 1, M, bvc, ST(L + 1), t->dyh + 2, nullptr, st);
-    {
-        const int chunks = (M + kRowsPerChunk - 1) / kRowsPerChunk;
-        colred_partial_kernel<kHeadConvGrad><<<chunks, 256, 0, st>>>(tower, nullptr, t->dyh, F, 3, F, M, nullptr, nullptr, t->part);
-        colred_finalize_kernel<kHeadConvGrad><<<(F + 255) / 256, 256, 0, st>>>(t->part, chunks, F, M, BnRef{t->off_pc, t->off_vc, F},
-                                                                               nullptr, nullptr, nullptr, t->stat, t->grad);
-        head_conv_dgrad_kernel<<<grid_for(MF), 256, 0, st>>>(t->dyh, t->blob, t->off_pc, t->off_vc, F, M, t->g);
-    }
-    RZ_LAUNCH_CHECK();
-
-    // tower backward; t->g holds the gradient of the current block's output
-    for (int i = R - 1; i >= 0; --i) {
-        const int l1 = 1 + 2 * i, l2 = l1 + 1;
-        bn_backward(t, t->g, A(l2), Y(l2), F, F, M, bnref(l2), ST(l2), t->dy, t->dz, st);
-        RZ_TRY(launch_wgrad(t, A(l1), F, F, t->dy, M, t->grad + t->conv_off[l2], st));
-        RZ_TRY(launch_conv(t->dy, F, t->wt + (size_t)(l2 - 1) * 9 * F * F, F, nullptr, nullptr, t->g1, M, st));
-        bn_backward(t, t->g1, A(l1), Y(l1), F, F, M, bnref(l1), ST(l1), t->dy, nullptr, st);
-        RZ_TRY(launch_wgrad(t, A(l1 - 1), F, F, t->dy, M, t->grad + t->conv_off[l1], st));
-        RZ_TRY(launch_conv(t->dy, F, t->wt + (size_t)(l1 - 1) * 9 * F * F, F, nullptr, t->dz, t->g, M, st));
-    }
-    bn_backward(t, t->g, A(0), Y(0), F, F, M, bnref(0), ST(0), t->dy, nullptr, st);
-    RZ_TRY(launch_wgrad(t, t->x0, kCin0, 2, t->dy, M, t->grad + t->conv_off[0], st));
-
-    update_kernel<<<kUpdateBlocks, 256, 0, st>>>(t->blob, t->vel, t->grad, t->stat, t->kind, t->n, lr, t->cfg.momentum, t->cfg.l2_reg,
-                                                  t->cfg.bn_momentum, t->bad, t->l2_part);
-    loss_kernel<<<1, 32, 0, st>>>(t->l2_part, t->loss_pv, t->cfg.l2_reg, t->bad, loss);
-    RZ_LAUNCH_CHECK();
-    return RZ_OK;
-}
-
-// ---- data-parallel group step ----------------------------------------------------------------------------------------
-// The step of trainer_step with the batch split into the shards of shard_plan, one per replica, and the same operations
-// in the same order on every sum the one-device step takes over the batch:
+// ---- the training step -----------------------------------------------------------------------------------------------
+// One schedule for a single trainer and for a data-parallel group.  The batch is split into the shards of shard_plan, one
+// per replica, and every sum over the batch is taken by the same operations in the same order whatever the split:
 //  * column reductions (BN statistics, BN and head-conv gradients): every replica writes the per-record partials of its
 //    shard; the primary gathers them into its `part` in batch order and runs the finalize over all chunks with the global
 //    M; the replicas copy back the finalized mean / invstd / sums (and the batch statistics of the moving averages);
@@ -860,38 +783,53 @@ int trainer_step(rz_trainer* t, const uint8_t* planes, const float* policy, cons
 // replica waiting on the primary, so no buffer a copy reads is rewritten before the copy has run; the replicas join the
 // caller's stream at the end and wait on it at the start.  A replica with an empty shard launches nothing but its copy
 // of the moving-average statistics, the gradient copy and update_kernel.
-int group_step(rz_trainer* t, const uint8_t* planes, const float* policy, const float* z, const int32_t* index, size_t n_records,
-               int batch, float lr, float* loss, cudaStream_t st) {
+// The primary's shard starts the batch, so it reads the caller's dataset through the caller's index; replicas 1.. read
+// records the primary staged for them.  A single trainer is the group of one replica: its shard is the batch, every
+// exchange is a loop over no replica, and it enqueues no staging, event or copy.  Its weight-gradient partials need no
+// slot either: each layer's go to `wpart` and are reduced at once.
+int step(rz_trainer* t, const uint8_t* planes, const float* policy, const float* z, const int32_t* index, size_t n_records, int batch,
+         float lr, float* loss, cudaStream_t st) {
     const int F = t->F, R = t->R, L = t->L, V = t->V, n = (int)t->reps.size(), Mg = batch * 64;
     int bounds[65];
     shard_plan(F, R, batch, n, bounds);
     const int per = wgrad_per(R ? F : kCin0, F, batch), per0 = wgrad_per(kCin0, F, batch);
-    auto on = [&](int r) { return cudaSetDevice(t->reps[r]->device); };
+    auto on = [&](int r) { return n > 1 ? cudaSetDevice(t->reps[r]->device) : cudaSuccess; };  // alone, t's device is current
     auto S = [&](int r) { return r ? t->reps[r]->stream : st; };
     auto b0 = [&](int r) { return bounds[r]; };
     auto nr = [&](int r) { return bounds[r + 1] - bounds[r]; };
-    auto Y = [&](rz_trainer* p, int l) { return p->y + (size_t)l * 64 * p->act * F; };
-    auto A = [&](rz_trainer* p, int l) { return p->a + (size_t)l * 64 * p->act * F; };
+    auto records = [&](int r) {
+        const rz_trainer* p = t->reps[r];
+        return r ? Records{p->sp, p->spol, p->sz, p->iota, p->act} : Records{planes, policy, z, index, n_records};
+    };
+    auto at = [&](rz_trainer* p, Operand o) { return o.buf ? p->*o.buf + (size_t)o.layer * 64 * p->act * F + o.col : nullptr; };
+    auto Y = [](int l) { return Operand{&rz_trainer::y, l}; };
+    auto A = [](int l) { return Operand{&rz_trainer::a, l}; };
+    const Operand none{}, g{&rz_trainer::g}, g1{&rz_trainer::g1}, dy{&rz_trainer::dy}, dz{&rz_trainer::dz};
+    const Operand hc{&rz_trainer::hc}, ah{&rz_trainer::ah}, dh{&rz_trainer::dh}, dyh{&rz_trainer::dyh};
+    auto value = [](Operand o) { return Operand{o.buf, 0, 2}; };  // the value head's column of a [M][3] head tensor
     auto ST = [&](rz_trainer* p, int l) { return p->stats + (size_t)l * 4 * F; };
     auto bnref = [&](int l) { return BnRef{t->conv_off[l], (size_t)9 * (l ? F : 2) * F, F}; };
     auto peer = [&](void* dst, int r_dst, const void* src, int r_src, size_t bytes, cudaStream_t s) {
         return bytes ? cudaMemcpyPeerAsync(dst, t->reps[r_dst]->device, src, t->reps[r_src]->device, bytes, s) : cudaSuccess;
     };
     const int chunks = batch;  // kRowsPerChunk = 64 rows: one column-reduction partial per record
-    // the capacities rz_trainer_create_group computed: a shard and its conv0 overflow fit the replica's buffers, and
-    // every layer's split partials fit one gradient slot
+    // the capacities the trainer was created with: a shard and its conv0 overflow fit the replica's buffers, and every
+    // layer's split partials fit `wpart` and one gradient slot
     for (int r = 0; r < n; ++r)
         RZ_REQUIRE((size_t)nr(r) + conv0_share(F, batch, b0(r), nr(r)).ov <= t->reps[r]->act,
-                   "group step: shard of replica %d exceeds its buffers", r);
+                   "training step: shard of replica %d exceeds its buffers", r);
     RZ_REQUIRE((size_t)((batch + per - 1) / per) * 9 * (R ? F : kCin0) * F <= t->wslot &&
                    (size_t)((batch + per0 - 1) / per0) * 9 * kCin0 * F <= t->wslot,
-               "group step: weight-gradient splits exceed the gradient slot");
+               "training step: weight-gradient splits exceed their scratch");
 
-    // stage the batch on the primary; each replica copies its shard (and conv0's overflow records) and expands x0
+    // the primary stages the batch for replicas 1.., which copy their shard (and conv0's overflow records); every
+    // replica expands its x0
     RZ_CUDA_TRY(cudaMemsetAsync(t->bad, 0, sizeof(int), st));
-    stage_kernel<<<(Mg + 255) / 256, 256, 0, st>>>(planes, policy, z, index, n_records, batch, t->sp, t->spol, t->sz, t->bad);
-    RZ_LAUNCH_CHECK();
-    RZ_CUDA_TRY(cudaEventRecord(t->ev, st));
+    if (n > 1) {
+        stage_kernel<<<(Mg + 255) / 256, 256, 0, st>>>(planes, policy, z, index, n_records, batch, t->sp, t->spol, t->sz, t->bad);
+        RZ_LAUNCH_CHECK();
+        RZ_CUDA_TRY(cudaEventRecord(t->ev, st));
+    }
     for (int r = 0; r < n; ++r) {
         rz_trainer* p = t->reps[r];
         const cudaStream_t s = S(r);
@@ -904,7 +842,8 @@ int group_step(rz_trainer* t, const uint8_t* planes, const float* policy, const 
             RZ_CUDA_TRY(peer(p->sz, r, t->sz + b0(r), 0, (size_t)rows * sizeof(float), s));
         }
         if (!nr(r)) continue;
-        gather_kernel<<<(rows * 64 * kCin0 + 255) / 256, 256, 0, s>>>(p->sp, p->iota, p->act, rows, p->x0, p->bad);
+        const Records rec = records(r);
+        gather_kernel<<<(rows * 64 * kCin0 + 255) / 256, 256, 0, s>>>(rec.planes, rec.index, rec.n, rows, p->x0, p->bad);
         pack_w0_kernel<<<(9 * kCin0 * F + 255) / 256, 256, 0, s>>>(p->blob + t->conv_off[0], F, p->w0p);
         for (int l = 1; l < L; ++l)
             pack_wt_kernel<<<grid_for((size_t)9 * F * F), 256, 0, s>>>(p->blob + t->conv_off[l], F, p->wt + (size_t)(l - 1) * 9 * F * F);
@@ -928,6 +867,7 @@ int group_step(rz_trainer* t, const uint8_t* planes, const float* policy, const 
     // after the primary's finalize: the replicas wait for it and copy layer l's finalized statistics (those with an empty
     // shard never read them) and the `stat_n` moving-average batch statistics at stat_off (which update_kernel reads)
     auto release = [&](int l, size_t stat_off, size_t stat_n) -> int {
+        if (n == 1) return RZ_OK;
         RZ_CUDA_TRY(on(0));
         RZ_CUDA_TRY(cudaEventRecord(t->ev, st));
         for (int r = 1; r < n; ++r) {
@@ -950,30 +890,35 @@ int group_step(rz_trainer* t, const uint8_t* planes, const float* policy, const 
         }
         return RZ_OK;
     };
-    // training-mode BN forward of layer slot l: yp(p) [rows][ld], res(p) nullable, out(p)
-    auto bn_forward_g = [&](auto yp, auto res, int ld, int C, BnRef bn, int l, auto out) -> int {
+    // training-mode BN forward of layer slot l over channels [0, C) of yp [rows][ld]: statistics, then normalise
+    // (+ residual `res`) + ReLU into out
+    auto bn_forward = [&](Operand yp, Operand res, int ld, int C, BnRef bn, int l, Operand out) -> int {
         RZ_TRY(partial_each([&](int, rz_trainer* p, int M, cudaStream_t s) {
-            colred_partial_kernel<kSum><<<chunks_of(M), 256, 0, s>>>(yp(p), nullptr, nullptr, ld, 0, C, M, nullptr, nullptr, p->part);
+            colred_partial_kernel<kSum><<<chunks_of(M), 256, 0, s>>>(at(p, yp), nullptr, nullptr, ld, 0, C, M, nullptr, nullptr, p->part);
         }));
         RZ_TRY(gather_part(C));
         colred_finalize_kernel<kSum><<<1, 256, 0, st>>>(t->part, chunks, C, Mg, bn, ST(t, l), ST(t, l) + F, nullptr, t->stat, t->grad);
         RZ_LAUNCH_CHECK();
         RZ_TRY(release(l, 0, 0));
         RZ_TRY(partial_each([&](int, rz_trainer* p, int M, cudaStream_t s) {
-            colred_partial_kernel<kSqDev><<<chunks_of(M), 256, 0, s>>>(yp(p), nullptr, nullptr, ld, 0, C, M, ST(p, l), nullptr, p->part);
+            colred_partial_kernel<kSqDev><<<chunks_of(M), 256, 0, s>>>(at(p, yp), nullptr, nullptr, ld, 0, C, M, ST(p, l), nullptr, p->part);
         }));
         RZ_TRY(gather_part(C));
         colred_finalize_kernel<kSqDev><<<1, 256, 0, st>>>(t->part, chunks, C, Mg, bn, ST(t, l), ST(t, l) + F, nullptr, t->stat, t->grad);
         RZ_LAUNCH_CHECK();
         RZ_TRY(release(l, bn.off + bn.kf + 3 * (size_t)bn.C, 2 * (size_t)bn.C));
         return partial_each([&](int, rz_trainer* p, int M, cudaStream_t s) {
-            bn_apply_kernel<<<grid_for((size_t)M * C), 256, 0, s>>>(yp(p), res(p), ld, C, M, p->blob, bn, ST(p, l), ST(p, l) + F, out(p));
+            bn_apply_kernel<<<grid_for((size_t)M * C), 256, 0, s>>>(at(p, yp), at(p, res), ld, C, M, p->blob, bn, ST(p, l), ST(p, l) + F,
+                                                                  at(p, out));
         });
     };
-    // BN + ReLU backward of layer slot l (bn_backward)
-    auto bn_backward_g = [&](auto gp, auto ap, auto yp, int ld, int C, BnRef bn, int l, auto dyp, auto dz_out) -> int {
+    // BN + ReLU backward of layer slot l: gp = gradient of the layer output ap; writes dyp (gradient of the conv output yp)
+    // and, when dz_out is given, the gradient below the ReLU (what the skip connection carries); the gamma / beta
+    // gradients go into the primary's grad
+    auto bn_backward = [&](Operand gp, Operand ap, Operand yp, int ld, int C, BnRef bn, int l, Operand dyp, Operand dz_out) -> int {
         RZ_TRY(partial_each([&](int, rz_trainer* p, int M, cudaStream_t s) {
-            colred_partial_kernel<kBnGrad><<<chunks_of(M), 256, 0, s>>>(yp(p), ap(p), gp(p), ld, 0, C, M, ST(p, l), ST(p, l) + F, p->part);
+            colred_partial_kernel<kBnGrad><<<chunks_of(M), 256, 0, s>>>(at(p, yp), at(p, ap), at(p, gp), ld, 0, C, M, ST(p, l), ST(p, l) + F,
+                                                                      p->part);
         }));
         RZ_TRY(gather_part(2 * (size_t)C));
         colred_finalize_kernel<kBnGrad><<<1, 256, 0, st>>>(t->part, chunks, C, Mg, bn, ST(t, l), ST(t, l) + F, ST(t, l) + 2 * F, t->stat,
@@ -981,47 +926,49 @@ int group_step(rz_trainer* t, const uint8_t* planes, const float* policy, const 
         RZ_LAUNCH_CHECK();
         RZ_TRY(release(l, 0, 0));
         return partial_each([&](int, rz_trainer* p, int M, cudaStream_t s) {
-            bn_backward_kernel<<<grid_for((size_t)M * C), 256, 0, s>>>(gp(p), ap(p), yp(p), ld, C, M, Mg, p->blob, bn, ST(p, l), ST(p, l) + F,
-                                                                     ST(p, l) + 2 * F, dyp(p), dz_out(p));
+            bn_backward_kernel<<<grid_for((size_t)M * C), 256, 0, s>>>(at(p, gp), at(p, ap), at(p, yp), ld, C, M, Mg, p->blob, bn, ST(p, l),
+                                                                     ST(p, l) + F, ST(p, l) + 2 * F, at(p, dyp), at(p, dz_out));
         });
     };
-    auto none = [](rz_trainer*) { return (float*)nullptr; };
-    // split partials of layer l's weight gradient: the primary writes into its slot, a replica into its wpart and on
-    auto wgrad_g = [&](int l, int r, const float* in, int cin, const float* dyp, int rows, int z0, int nz, int per_l) -> int {
+    // split partials [z0, z0 + nz) of layer l's weight gradient, computed by replica r from its rows `in` and `dyp`.  A
+    // single replica reduces them at once from its wpart.  In a group the primary writes into the layer's slot and a
+    // replica into its wpart and on, and every layer is reduced after the join.
+    auto wgrad = [&](int l, int r, const float* in, const float* dyp, int rows, int z0, int nz) -> int {
         if (!nz) return RZ_OK;
         rz_trainer* p = t->reps[r];
+        const int cin = l ? F : kCin0;
         const size_t slice = (size_t)9 * cin * F;
-        float* dst = t->wgather + (size_t)l * t->wslot + (size_t)z0 * slice;
-        dim3 grid((9 * cin + kBM - 1) / kBM, (F + kBN - 1) / kBN, nz);
-        conv_gemm_tf32_kernel<true><<<grid, 256, 0, S(r)>>>(in, cin, dyp, F, nullptr, nullptr, r ? p->wpart : dst, rows * 64, per_l * 64);
-        RZ_LAUNCH_CHECK();
-        if (r) RZ_CUDA_TRY(peer(dst, 0, p->wpart, r, (size_t)nz * slice * sizeof(float), S(r)));
+        float* slot = n > 1 ? t->wgather + (size_t)l * t->wslot + (size_t)z0 * slice : nullptr;
+        RZ_TRY(launch_wgrad(in, cin, l ? F : 2, dyp, F, rows, nz, l ? per : per0, slot && !r ? slot : p->wpart,
+                            slot ? nullptr : t->grad + t->conv_off[l], S(r)));
+        if (r) RZ_CUDA_TRY(peer(slot, 0, p->wpart, r, (size_t)nz * slice * sizeof(float), S(r)));
         return RZ_OK;
     };
 
     // forward
     for (int l = 0; l < L; ++l) {
         RZ_TRY(partial_each([&](int, rz_trainer* p, int M, cudaStream_t s) {
-            const float* in = l ? A(p, l - 1) : p->x0;
+            const float* in = l ? at(p, A(l - 1)) : p->x0;
             const float* w = l ? p->blob + t->conv_off[l] : p->w0p;
-            return launch_conv(in, l ? F : kCin0, w, F, p->blob + t->conv_off[l] + bnref(l).kf, nullptr, Y(p, l), M, s);
+            return launch_conv(in, l ? F : kCin0, w, F, p->blob + t->conv_off[l] + bnref(l).kf, nullptr, at(p, Y(l)), M, s);
         }));
-        RZ_TRY(bn_forward_g([&](rz_trainer* p) { return Y(p, l); },
-                            [&](rz_trainer* p) { return (l >= 2 && l % 2 == 0) ? A(p, l - 2) : nullptr; }, F, F, bnref(l), l,
-                            [&](rz_trainer* p) { return A(p, l); }));
+        const Operand res = (l >= 2 && l % 2 == 0) ? A(l - 2) : none;  // conv2 of a block adds the block input
+        RZ_TRY(bn_forward(Y(l), res, F, F, bnref(l), l, A(l)));
     }
+    const Operand tower = A(L - 1);
     RZ_TRY(partial_each([&](int, rz_trainer* p, int M, cudaStream_t s) {
-        head_conv_kernel<<<(M * 32 + 255) / 256, 256, 0, s>>>(A(p, L - 1), F, M, p->blob, t->off_pc, t->off_vc, p->hc);
+        head_conv_kernel<<<(M * 32 + 255) / 256, 256, 0, s>>>(at(p, tower), F, M, p->blob, t->off_pc, t->off_vc, p->hc);
     }));
     const BnRef bpc{t->off_pc, (size_t)F * 2, 2}, bvc{t->off_vc, (size_t)F, 1};
-    RZ_TRY(bn_forward_g([](rz_trainer* p) { return p->hc; }, none, 3, 2, bpc, L, [](rz_trainer* p) { return p->ah; }));
-    RZ_TRY(bn_forward_g([](rz_trainer* p) { return p->hc + 2; }, none, 3, 1, bvc, L + 1, [](rz_trainer* p) { return p->ah + 2; }));
+    RZ_TRY(bn_forward(hc, none, 3, 2, bpc, L, ah));
+    RZ_TRY(bn_forward(value(hc), none, 3, 1, bvc, L + 1, value(ah)));
 
     // loss and head backward; the per-record head tensors go to the primary
     const size_t fc_smem = head_fc_smem(V);
-    RZ_TRY(partial_each([&](int, rz_trainer* p, int M, cudaStream_t s) {
-        head_fc_kernel<<<M / 64, 256, fc_smem, s>>>(p->ah, p->blob, t->ho, V, p->spol, p->sz, p->iota, p->act, batch, p->hp, p->hv, p->dl,
-                                                    p->h1, p->dh1, p->dv, p->lp, p->lv, p->dh);
+    RZ_TRY(partial_each([&](int r, rz_trainer* p, int M, cudaStream_t s) {
+        const Records rec = records(r);
+        head_fc_kernel<<<M / 64, 256, fc_smem, s>>>(p->ah, p->blob, t->ho, V, rec.policy, rec.z, rec.index, rec.n, batch, p->hp, p->hv,
+                                                    p->dl, p->h1, p->dh1, p->dv, p->lp, p->lv, p->dh);
     }));
     for (int r = 1; r < n; ++r) {
         RZ_CUDA_TRY(on(r));
@@ -1046,12 +993,10 @@ int group_step(rz_trainer* t, const uint8_t* planes, const float* policy, const 
     head_fc_grad_kernel<<<(n_fc + 255) / 256, 256, 0, st>>>(t->hp, t->hv, t->dl, t->h1, t->dh1, t->dv, t->lp, t->lv, V, batch, t->ho,
                                                             t->grad, t->loss_pv);
     RZ_LAUNCH_CHECK();
-    RZ_TRY(bn_backward_g([](rz_trainer* p) { return p->dh; }, [](rz_trainer* p) { return p->ah; }, [](rz_trainer* p) { return p->hc; },
-                         3, 2, bpc, L, [](rz_trainer* p) { return p->dyh; }, none));
-    RZ_TRY(bn_backward_g([](rz_trainer* p) { return p->dh + 2; }, [](rz_trainer* p) { return p->ah + 2; },
-                         [](rz_trainer* p) { return p->hc + 2; }, 3, 1, bvc, L + 1, [](rz_trainer* p) { return p->dyh + 2; }, none));
+    RZ_TRY(bn_backward(dh, ah, hc, 3, 2, bpc, L, dyh, none));
+    RZ_TRY(bn_backward(value(dh), value(ah), value(hc), 3, 1, bvc, L + 1, value(dyh), none));
     RZ_TRY(partial_each([&](int, rz_trainer* p, int M, cudaStream_t s) {
-        colred_partial_kernel<kHeadConvGrad><<<chunks_of(M), 256, 0, s>>>(A(p, L - 1), nullptr, p->dyh, F, 3, F, M, nullptr, nullptr, p->part);
+        colred_partial_kernel<kHeadConvGrad><<<chunks_of(M), 256, 0, s>>>(at(p, tower), nullptr, p->dyh, F, 3, F, M, nullptr, nullptr, p->part);
     }));
     RZ_TRY(gather_part(3 * (size_t)F));
     colred_finalize_kernel<kHeadConvGrad><<<(F + 255) / 256, 256, 0, st>>>(t->part, chunks, F, Mg, BnRef{t->off_pc, t->off_vc, F}, nullptr,
@@ -1062,36 +1007,33 @@ int group_step(rz_trainer* t, const uint8_t* planes, const float* policy, const 
         head_conv_dgrad_kernel<<<grid_for((size_t)M * F), 256, 0, s>>>(p->dyh, p->blob, t->off_pc, t->off_vc, F, M, p->g);
     }));
 
-    // tower backward
-    auto tower_wgrad = [&](int l, auto in) -> int {
+    // tower backward; g holds the gradient of the current block's output
+    auto tower_wgrad = [&](int l, Operand in) -> int {
         for (int r = 0; r < n; ++r) {
             if (!nr(r)) continue;
             RZ_CUDA_TRY(on(r));
             rz_trainer* p = t->reps[r];
-            RZ_TRY(wgrad_g(l, r, in(p), F, p->dy, nr(r), b0(r) / per, (nr(r) + per - 1) / per, per));
+            RZ_TRY(wgrad(l, r, at(p, in), p->dy, nr(r), b0(r) / per, (nr(r) + per - 1) / per));
         }
         return RZ_OK;
     };
-    auto dgrad = [&](int l, auto add, auto out) {
+    auto dgrad = [&](int l, Operand add, Operand out) {
         return partial_each([&](int, rz_trainer* p, int M, cudaStream_t s) {
-            return launch_conv(p->dy, F, p->wt + (size_t)(l - 1) * 9 * F * F, F, nullptr, add(p), out(p), M, s);
+            return launch_conv(p->dy, F, p->wt + (size_t)(l - 1) * 9 * F * F, F, nullptr, at(p, add), at(p, out), M, s);
         });
     };
     for (int i = R - 1; i >= 0; --i) {
         const int l1 = 1 + 2 * i, l2 = l1 + 1;
-        RZ_TRY(bn_backward_g([](rz_trainer* p) { return p->g; }, [&](rz_trainer* p) { return A(p, l2); }, [&](rz_trainer* p) { return Y(p, l2); },
-                             F, F, bnref(l2), l2, [](rz_trainer* p) { return p->dy; }, [](rz_trainer* p) { return p->dz; }));
-        RZ_TRY(tower_wgrad(l2, [&](rz_trainer* p) { return A(p, l1); }));
-        RZ_TRY(dgrad(l2, none, [](rz_trainer* p) { return p->g1; }));
-        RZ_TRY(bn_backward_g([](rz_trainer* p) { return p->g1; }, [&](rz_trainer* p) { return A(p, l1); }, [&](rz_trainer* p) { return Y(p, l1); },
-                             F, F, bnref(l1), l1, [](rz_trainer* p) { return p->dy; }, none));
-        RZ_TRY(tower_wgrad(l1, [&](rz_trainer* p) { return A(p, l1 - 1); }));
-        RZ_TRY(dgrad(l1, [](rz_trainer* p) { return p->dz; }, [](rz_trainer* p) { return p->g; }));
+        RZ_TRY(bn_backward(g, A(l2), Y(l2), F, F, bnref(l2), l2, dy, dz));
+        RZ_TRY(tower_wgrad(l2, A(l1)));
+        RZ_TRY(dgrad(l2, none, g1));
+        RZ_TRY(bn_backward(g1, A(l1), Y(l1), F, F, bnref(l1), l1, dy, none));
+        RZ_TRY(tower_wgrad(l1, A(l1 - 1)));
+        RZ_TRY(dgrad(l1, dz, g));
     }
-    RZ_TRY(bn_backward_g([](rz_trainer* p) { return p->g; }, [&](rz_trainer* p) { return A(p, 0); }, [&](rz_trainer* p) { return Y(p, 0); },
-                         F, F, bnref(0), 0, [](rz_trainer* p) { return p->dy; }, none));
+    RZ_TRY(bn_backward(g, A(0), Y(0), F, F, bnref(0), 0, dy, none));
     // conv0: a split that straddles the end of shard r takes the first rows of layer 0's dy from replica r + 1 (the x0
-    // rows came with the staged records)
+    // rows came with the replica's own records)
     Conv0Share c0[64];
     for (int r = 0; r < n; ++r) c0[r] = conv0_share(F, batch, b0(r), nr(r));
     for (int r = 1; r < n; ++r) {
@@ -1106,37 +1048,37 @@ int group_step(rz_trainer* t, const uint8_t* planes, const float* policy, const 
         RZ_CUDA_TRY(on(r));
         rz_trainer* p = t->reps[r];
         if (c0[r].ov) RZ_CUDA_TRY(cudaStreamWaitEvent(S(r), t->reps[r + 1]->ev, 0));
-        RZ_TRY(wgrad_g(0, r, p->x0 + (size_t)c0[r].row0 * 64 * kCin0, kCin0, p->dy + (size_t)c0[r].row0 * 64 * F, c0[r].rows, c0[r].z0,
-                       c0[r].nz, per0));
+        RZ_TRY(wgrad(0, r, p->x0 + (size_t)c0[r].row0 * 64 * kCin0, p->dy + (size_t)c0[r].row0 * 64 * F, c0[r].rows, c0[r].z0, c0[r].nz));
     }
 
-    // join the replicas' partials, reduce every layer in split order, hand the gradient out, update everywhere
-    for (int r = 1; r < n; ++r) {
-        RZ_CUDA_TRY(on(r));
-        RZ_CUDA_TRY(cudaEventRecord(t->reps[r]->ev, S(r)));
-    }
-    RZ_CUDA_TRY(on(0));
-    for (int r = 1; r < n; ++r) RZ_CUDA_TRY(cudaStreamWaitEvent(st, t->reps[r]->ev, 0));
-    for (int l = 0; l < L; ++l) {
-        const int cin = l ? F : kCin0, pl = l ? per : per0;
-        wgrad_reduce_kernel<<<grid_for((size_t)9 * cin * F), 256, 0, st>>>(t->wgather + (size_t)l * t->wslot, (batch + pl - 1) / pl, cin,
-                                                                           l ? F : 2, F, t->grad + t->conv_off[l]);
-    }
-    RZ_LAUNCH_CHECK();
-    RZ_CUDA_TRY(cudaEventRecord(t->ev, st));
-    for (int r = 1; r < n; ++r) {
-        rz_trainer* p = t->reps[r];
-        RZ_CUDA_TRY(on(r));
-        RZ_CUDA_TRY(cudaStreamWaitEvent(p->stream, t->ev, 0));
-        RZ_CUDA_TRY(peer(p->grad, r, t->grad, 0, t->n * sizeof(float), p->stream));
-        RZ_CUDA_TRY(peer(p->bad, r, t->bad, 0, sizeof(int), p->stream));
-        update_kernel<<<kUpdateBlocks, 256, 0, p->stream>>>(p->blob, p->vel, p->grad, p->stat, p->kind, t->n, lr, t->cfg.momentum,
-                                                            t->cfg.l2_reg, t->cfg.bn_momentum, p->bad, p->l2_part);
+    if (n > 1) {  // join the replicas' partials, reduce every layer in split order, hand the gradient out, update the replicas
+        for (int r = 1; r < n; ++r) {
+            RZ_CUDA_TRY(on(r));
+            RZ_CUDA_TRY(cudaEventRecord(t->reps[r]->ev, S(r)));
+        }
+        RZ_CUDA_TRY(on(0));
+        for (int r = 1; r < n; ++r) RZ_CUDA_TRY(cudaStreamWaitEvent(st, t->reps[r]->ev, 0));
+        for (int l = 0; l < L; ++l) {
+            const int cin = l ? F : kCin0, pl = l ? per : per0;
+            wgrad_reduce_kernel<<<grid_for((size_t)9 * cin * F), 256, 0, st>>>(t->wgather + (size_t)l * t->wslot, (batch + pl - 1) / pl, cin,
+                                                                               l ? F : 2, F, t->grad + t->conv_off[l]);
+        }
         RZ_LAUNCH_CHECK();
-        RZ_CUDA_TRY(cudaEventRecord(p->ev, p->stream));
+        RZ_CUDA_TRY(cudaEventRecord(t->ev, st));
+        for (int r = 1; r < n; ++r) {
+            rz_trainer* p = t->reps[r];
+            RZ_CUDA_TRY(on(r));
+            RZ_CUDA_TRY(cudaStreamWaitEvent(p->stream, t->ev, 0));
+            RZ_CUDA_TRY(peer(p->grad, r, t->grad, 0, t->n * sizeof(float), p->stream));
+            RZ_CUDA_TRY(peer(p->bad, r, t->bad, 0, sizeof(int), p->stream));
+            update_kernel<<<kUpdateBlocks, 256, 0, p->stream>>>(p->blob, p->vel, p->grad, p->stat, p->kind, t->n, lr, t->cfg.momentum,
+                                                                t->cfg.l2_reg, t->cfg.bn_momentum, p->bad, p->l2_part);
+            RZ_LAUNCH_CHECK();
+            RZ_CUDA_TRY(cudaEventRecord(p->ev, p->stream));
+        }
+        RZ_CUDA_TRY(on(0));
+        for (int r = 1; r < n; ++r) RZ_CUDA_TRY(cudaStreamWaitEvent(st, t->reps[r]->ev, 0));  // update_kernel rewrites grad
     }
-    RZ_CUDA_TRY(on(0));
-    for (int r = 1; r < n; ++r) RZ_CUDA_TRY(cudaStreamWaitEvent(st, t->reps[r]->ev, 0));  // update_kernel rewrites grad
     update_kernel<<<kUpdateBlocks, 256, 0, st>>>(t->blob, t->vel, t->grad, t->stat, t->kind, t->n, lr, t->cfg.momentum, t->cfg.l2_reg,
                                                   t->cfg.bn_momentum, t->bad, t->l2_part);
     loss_kernel<<<1, 32, 0, st>>>(t->l2_part, t->loss_pv, t->cfg.l2_reg, t->bad, loss);
@@ -1156,7 +1098,8 @@ int check_cfg(const rz_net_cfg* net, const rz_train_cfg* cfg) {
 }
 
 // A trainer, or one replica of a group: activation and backward buffers for `act` records, the batch-wide buffers (column
-// partials, per-record head tensors, staged records) for `full`.  A single trainer has act = full = max_batch.
+// partials, per-record head tensors, staged records) for `full`.  A single trainer has act = full = max_batch and, with
+// no replica to exchange with, no staged records, identity index, gradient slots, stream or event.
 int trainer_create(const rz_net_cfg* net, const rz_train_cfg* cfg, int device, size_t act, size_t full, bool group, bool primary,
                    rz_trainer** out) {
     RZ_CUDA_TRY(cudaSetDevice(device));
@@ -1191,30 +1134,30 @@ int trainer_create(const rz_net_cfg* net, const rz_train_cfg* cfg, int device, s
     t->n = kind.size();
 
     const size_t B = full, M = 64 * act, MF = M * F, L = t->L;
-    t->wgrad_splits_max = wgrad_splits(F, F, cfg->max_batch);
-    const int s0 = wgrad_splits(kCin0, F, cfg->max_batch);
-    const size_t wpart = std::max((size_t)t->wgrad_splits_max * 9 * F * F, (size_t)s0 * 9 * kCin0 * F);
+    const int splits = wgrad_splits(F, F, cfg->max_batch), splits0 = wgrad_splits(kCin0, F, cfg->max_batch);
+    t->wslot = std::max((size_t)splits * 9 * F * F, (size_t)splits0 * 9 * kCin0 * F);
     struct { float** p; size_t n; } allocs[] = {
         {&t->blob, t->n}, {&t->vel, t->n}, {&t->grad, t->n}, {&t->stat, t->n}, {&t->x0, M * kCin0}, {&t->w0p, (size_t)9 * kCin0 * F},
         {&t->wt, (size_t)std::max(2 * R, 1) * 9 * F * F}, {&t->y, L * MF}, {&t->a, L * MF}, {&t->g, MF}, {&t->g1, MF}, {&t->dy, MF},
         {&t->dz, MF}, {&t->hc, M * 3}, {&t->ah, M * 3}, {&t->dh, M * 3}, {&t->dyh, M * 3}, {&t->hp, B * 128}, {&t->hv, B * 64},
         {&t->dl, B * 64}, {&t->h1, B * V}, {&t->dh1, B * V}, {&t->dv, B}, {&t->lp, B}, {&t->lv, B}, {&t->stats, (L + 2) * 4 * F},
-        {&t->wpart, wpart}, {&t->l2_part, kUpdateBlocks}, {&t->loss_pv, 2}};
+        {&t->wpart, t->wslot}, {&t->l2_part, kUpdateBlocks}, {&t->loss_pv, 2}};
     cudaError_t e = cudaSuccess;
     for (auto& a : allocs)
         if (e == cudaSuccess) e = cudaMalloc(a.p, a.n * sizeof(float));
     if (group) {
-        t->wslot = wpart;
-        std::vector<int32_t> iota(act);
-        for (size_t i = 0; i < act; ++i) iota[i] = (int32_t)i;
         if (e == cudaSuccess) e = cudaMalloc(&t->sp, B * 128);
         if (e == cudaSuccess) e = cudaMalloc(&t->spol, B * 64 * sizeof(float));
         if (e == cudaSuccess) e = cudaMalloc(&t->sz, B * sizeof(float));
+        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&t->ev, cudaEventDisableTiming);
+        if (e == cudaSuccess && primary) e = cudaMalloc(&t->wgather, L * t->wslot * sizeof(float));
+    }
+    if (group && !primary) {
+        std::vector<int32_t> iota(act);
+        for (size_t i = 0; i < act; ++i) iota[i] = (int32_t)i;
         if (e == cudaSuccess) e = cudaMalloc(&t->iota, act * sizeof(int32_t));
         if (e == cudaSuccess) e = cudaMemcpy(t->iota, iota.data(), act * sizeof(int32_t), cudaMemcpyHostToDevice);
-        if (e == cudaSuccess && primary) e = cudaMalloc(&t->wgather, L * wpart * sizeof(float));
-        if (e == cudaSuccess && !primary) e = cudaStreamCreateWithFlags(&t->stream, cudaStreamNonBlocking);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&t->ev, cudaEventDisableTiming);
+        if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&t->stream, cudaStreamNonBlocking);
     }
     if (e == cudaSuccess) e = cudaMalloc(&t->part, B * 3 * F * sizeof(double));
     if (e == cudaSuccess) e = cudaMalloc(&t->kind, t->n);
@@ -1233,6 +1176,7 @@ int trainer_create(const rz_net_cfg* net, const rz_train_cfg* cfg, int device, s
         delete t;
         return RZ_ENOMEM;
     }
+    if (primary) t->reps.push_back(t);
     *out = t;
     return RZ_OK;
 }
@@ -1286,7 +1230,6 @@ int rz_trainer_create_group(const rz_net_cfg* net, const rz_train_cfg* cfg, cons
     }
     rz_trainer* t = nullptr;
     RZ_TRY(trainer_create(net, cfg, devices[0], act[0], cfg->max_batch, true, true, &t));
-    t->reps.push_back(t);
     for (int r = 1; r < n_devices; ++r) {
         rz_trainer* p = nullptr;
         const int rc = trainer_create(net, cfg, devices[r], act[r], act[r], true, false, &p);
@@ -1317,7 +1260,7 @@ int rz_trainer_blob_size(const rz_trainer* t, size_t* n_floats) {
 int rz_trainer_load_weights(rz_trainer* t, const float* blob_host, size_t n_floats) {
     RZ_REQUIRE(t && blob_host, "rz_trainer_load_weights: null pointer");
     RZ_REQUIRE(n_floats == t->n, "weight blob has %zu floats, this configuration needs %zu", n_floats, t->n);
-    for (rz_trainer* p : t->reps.empty() ? std::vector<rz_trainer*>{t} : t->reps) {
+    for (rz_trainer* p : t->reps) {
         RZ_CUDA_TRY(cudaSetDevice(p->device));
         RZ_CUDA_TRY(cudaMemcpy(p->blob, blob_host, n_floats * sizeof(float), cudaMemcpyHostToDevice));
         RZ_CUDA_TRY(cudaMemset(p->vel, 0, n_floats * sizeof(float)));
@@ -1359,8 +1302,7 @@ int rz_trainer_step_dev(rz_trainer* t, const uint8_t* planes, const float* polic
     RZ_REQUIRE(isfinite(lr), "rz_trainer_step_dev: non-finite learning rate");
     if (!t->loaded) { set_error("rz_trainer: weights not loaded"); return RZ_ESTATE; }
     RZ_CUDA_TRY(cudaSetDevice(t->device));
-    if (t->reps.empty()) return trainer_step(t, planes, policy, z, index, n_records, (int)batch, lr, loss_dev, (cudaStream_t)stream);
-    const int rc = group_step(t, planes, policy, z, index, n_records, (int)batch, lr, loss_dev, (cudaStream_t)stream);
+    const int rc = step(t, planes, policy, z, index, n_records, (int)batch, lr, loss_dev, (cudaStream_t)stream);
     cudaSetDevice(t->device);
     return rc;
 }
@@ -1368,9 +1310,9 @@ int rz_trainer_step_dev(rz_trainer* t, const uint8_t* planes, const float* polic
 int rz_trainer_replica_state_dev(rz_trainer* t, int r, float* blob_dev, float* vel_dev, size_t n_floats, void* stream) {
     RZ_REQUIRE(t && blob_dev && vel_dev, "rz_trainer_replica_state_dev: null pointer");
     RZ_REQUIRE(n_floats == t->n, "weight blob has %zu floats, this configuration needs %zu", n_floats, t->n);
-    const int n = t->reps.empty() ? 1 : (int)t->reps.size();
+    const int n = (int)t->reps.size();
     RZ_REQUIRE(r >= 0 && r < n, "rz_trainer_replica_state_dev: replica %d outside [0, %d)", r, n);
-    const rz_trainer* p = r ? t->reps[r] : t;
+    const rz_trainer* p = t->reps[r];
     RZ_CUDA_TRY(cudaSetDevice(t->device));
     RZ_CUDA_TRY(cudaMemcpyPeerAsync(blob_dev, t->device, p->blob, p->device, n_floats * sizeof(float), (cudaStream_t)stream));
     RZ_CUDA_TRY(cudaMemcpyPeerAsync(vel_dev, t->device, p->vel, p->device, n_floats * sizeof(float), (cudaStream_t)stream));
@@ -1410,8 +1352,9 @@ int rz_trainer_debug_conv_dev(rz_trainer* t, int op, const float* in, const floa
         case RZ_TRAIN_CONV_WGRAD:
         case RZ_TRAIN_CONV0_WGRAD: {
             RZ_REQUIRE(add && !kernel && !bias, "rz_trainer_debug_conv_dev: the weight gradient takes dy in `add`, no kernel or bias");
-            const bool c0 = op == RZ_TRAIN_CONV0_WGRAD;
-            return launch_wgrad(t, in, c0 ? kCin0 : F, c0 ? 2 : F, add, M, out, st);
+            const bool c0 = op == RZ_TRAIN_CONV0_WGRAD;  // all of the layer's splits at this batch, reduced at once as in the step
+            const int cin = c0 ? kCin0 : F, per = wgrad_per(cin, F, (int)batch);
+            return launch_wgrad(in, cin, c0 ? 2 : F, add, F, (int)batch, ((int)batch + per - 1) / per, per, t->wpart, out, st);
         }
         default:
             set_error("rz_trainer_debug_conv_dev: unknown op %d", op);
