@@ -443,6 +443,42 @@ int rz_trainer_replica_state_dev(rz_trainer* t, int r, float* blob_dev, float* v
 int rz_trainer_debug_conv_dev(rz_trainer* t, int op, const float* in, const float* kernel, const float* bias, const float* add,
                               size_t batch, float* out, void* stream);
 
+/* test hook: copy one intermediate tensor of the last step (batch B, M = 64 * B pixel rows, L = 1 + 2 * res_blocks tower
+ * layers) into out (device, exactly n_floats floats, stream-ordered after the step).  `layer` selects the tower layer
+ * of Y, A, G, DY and DZ, the statistics slot of STATS, and is 0 for the others.  Single trainers only: RZ_ESTATE on a
+ * group, before the first step, and for G / DY / DZ unless the last step ran with rz_trainer_debug_keep_backward on;
+ * RZ_EINVAL for an unknown tensor, a layer out of range or a wrong n_floats. */
+#define RZ_TRAIN_T_X0 0       /* [M][16] input planes, channels 2..15 zero */
+#define RZ_TRAIN_T_Y 1        /* [M][F] conv output of tower layer l (pre-BN, bias included) */
+#define RZ_TRAIN_T_A 2        /* [M][F] output of tower layer l (after BN, residual and ReLU) */
+#define RZ_TRAIN_T_STATS 3    /* [4][F] slot l in [0, L + 2) (L: policy head, L + 1: value head): batch mean [F],
+                                 invstd [F], then sum dz [C] and sum dz * xhat [C] packed after them, over the slot's
+                                 C channels (F in the tower, 2 and 1 in the heads) */
+#define RZ_TRAIN_T_STAT 4     /* [blob floats] the batch mean / biased variance the moving averages take, at the moving
+                                 statistics' blob offsets; 0 elsewhere */
+#define RZ_TRAIN_T_HC 5       /* [M][3] head 1x1 conv outputs (policy 0..1, value 2) */
+#define RZ_TRAIN_T_AH 6       /* [M][3] their BN + ReLU outputs */
+#define RZ_TRAIN_T_DH 7       /* [M][3] gradient of ah */
+#define RZ_TRAIN_T_DYH 8      /* [M][3] gradient of hc */
+#define RZ_TRAIN_T_HP 9       /* [B][128] policy Dense input (channels-first flatten of ah) */
+#define RZ_TRAIN_T_HV 10      /* [B][64] value Dense input */
+#define RZ_TRAIN_T_DL 11      /* [B][64] gradient of the logits */
+#define RZ_TRAIN_T_H1 12      /* [B][V] value hidden layer (after ReLU) */
+#define RZ_TRAIN_T_DH1 13     /* [B][V] its gradient below the ReLU */
+#define RZ_TRAIN_T_DV 14      /* [B] gradient of the value output before tanh */
+#define RZ_TRAIN_T_LP 15      /* [B] policy loss per record */
+#define RZ_TRAIN_T_LV 16      /* [B] value loss per record */
+#define RZ_TRAIN_T_LOSS_PV 17 /* [2] batch-mean policy and value loss */
+#define RZ_TRAIN_T_G 18       /* [M][F] gradient of A(l)        (backward taps) */
+#define RZ_TRAIN_T_DY 19      /* [M][F] gradient of Y(l)        (backward taps) */
+#define RZ_TRAIN_T_DZ 20      /* [M][F] gradient below the ReLU that the skip connection carries, conv2 layers
+                                 (l = 2, 4, ..) only        (backward taps) */
+int rz_trainer_debug_tensor_dev(rz_trainer* t, int which, int layer, float* out, size_t n_floats, void* stream);
+/* test hook: on != 0 allocates [L][3][64 * max_batch][F] floats and makes every following step copy each tower layer's
+ * G, DY and DZ there (three device-to-device copies per layer); 0 frees them, and the step enqueues nothing extra.
+ * RZ_ESTATE on a group. */
+int rz_trainer_debug_keep_backward(rz_trainer* t, int on);
+
 #ifdef __cplusplus
 }
 #endif

@@ -677,6 +677,11 @@ struct rz_trainer {
     float *spol, *sz;
     int32_t* iota;                // replicas 1..: identity index [act]: the staged records are the replica's dataset
     float* wgather;               // primary: every layer's weight-gradient split partials [L][wslot], reduced after the join
+
+    // test hooks of a single trainer (rz_trainer_debug_tensor_dev, rz_trainer_debug_keep_backward)
+    int last_batch;               // batch of the last step; 0 before the first
+    float* taps;                  // [L][3][64 * act][F]: each tower layer's G (gradient of A), dY and dz; null when off
+    bool taps_valid;              // the last step ran with the taps on
 };
 
 namespace {
@@ -684,7 +689,7 @@ namespace {
 void trainer_free(rz_trainer* t) {
     float* bufs[] = {t->blob, t->vel, t->grad, t->stat, t->x0, t->w0p, t->wt, t->y, t->a, t->g, t->g1, t->dy, t->dz, t->hc, t->ah,
                      t->dh, t->dyh, t->hp, t->hv, t->dl, t->h1, t->dh1, t->dv, t->lp, t->lv, t->stats, t->wpart,
-                     t->l2_part, t->loss_pv, t->spol, t->sz, t->wgather};
+                     t->l2_part, t->loss_pv, t->spol, t->sz, t->wgather, t->taps};
     for (float* p : bufs) cudaFree(p);
     cudaFree(t->part);
     cudaFree(t->kind);
@@ -821,6 +826,8 @@ int step(rz_trainer* t, const uint8_t* planes, const float* policy, const float*
     RZ_REQUIRE((size_t)((batch + per - 1) / per) * 9 * (R ? F : kCin0) * F <= t->wslot &&
                    (size_t)((batch + per0 - 1) / per0) * 9 * kCin0 * F <= t->wslot,
                "training step: weight-gradient splits exceed their scratch");
+    t->last_batch = batch;
+    t->taps_valid = t->taps != nullptr;
 
     // the primary stages the batch for replicas 1.., which copy their shard (and conv0's overflow records); every
     // replica expands its x0
@@ -925,10 +932,18 @@ int step(rz_trainer* t, const uint8_t* planes, const float* policy, const float*
                                                            t->grad);
         RZ_LAUNCH_CHECK();
         RZ_TRY(release(l, 0, 0));
-        return partial_each([&](int, rz_trainer* p, int M, cudaStream_t s) {
+        RZ_TRY(partial_each([&](int, rz_trainer* p, int M, cudaStream_t s) {
             bn_backward_kernel<<<grid_for((size_t)M * C), 256, 0, s>>>(at(p, gp), at(p, ap), at(p, yp), ld, C, M, Mg, p->blob, bn, ST(p, l),
                                                                      ST(p, l) + F, ST(p, l) + 2 * F, at(p, dyp), at(p, dz_out));
-        });
+        }));
+        if (t->taps && l < L) {  // test hook, single trainers only: keep this tower layer's G, dY and dz before they are reused
+            const size_t bytes = (size_t)Mg * F * sizeof(float), stride = (size_t)64 * t->act * F;
+            float* tap = t->taps + (size_t)l * 3 * stride;
+            RZ_CUDA_TRY(cudaMemcpyAsync(tap, at(t, gp), bytes, cudaMemcpyDeviceToDevice, st));
+            RZ_CUDA_TRY(cudaMemcpyAsync(tap + stride, at(t, dyp), bytes, cudaMemcpyDeviceToDevice, st));
+            if (dz_out.buf) RZ_CUDA_TRY(cudaMemcpyAsync(tap + 2 * stride, at(t, dz_out), bytes, cudaMemcpyDeviceToDevice, st));
+        }
+        return RZ_OK;
     };
     // split partials [z0, z0 + nz) of layer l's weight gradient, computed by replica r from its rows `in` and `dyp`.  A
     // single replica reduces them at once from its wpart.  In a group the primary writes into the layer's slot and a
@@ -1360,6 +1375,71 @@ int rz_trainer_debug_conv_dev(rz_trainer* t, int op, const float* in, const floa
             set_error("rz_trainer_debug_conv_dev: unknown op %d", op);
             return RZ_EINVAL;
     }
+}
+
+int rz_trainer_debug_keep_backward(rz_trainer* t, int on) {
+    RZ_REQUIRE(t, "rz_trainer_debug_keep_backward: null pointer");
+    if (t->reps.size() > 1) { set_error("rz_trainer_debug_keep_backward: not available on a data-parallel group"); return RZ_ESTATE; }
+    RZ_CUDA_TRY(cudaSetDevice(t->device));
+    t->taps_valid = false;
+    if (!on) {
+        RZ_CUDA_TRY(cudaFree(t->taps));
+        t->taps = nullptr;
+        return RZ_OK;
+    }
+    if (t->taps) return RZ_OK;
+    const size_t n = (size_t)t->L * 3 * 64 * t->act * t->F;
+    if (cudaMalloc(&t->taps, n * sizeof(float)) != cudaSuccess) {
+        cudaGetLastError();
+        t->taps = nullptr;
+        set_error("rz_trainer_debug_keep_backward: cannot allocate %zu floats", n);
+        return RZ_ENOMEM;
+    }
+    RZ_CUDA_TRY(cudaMemset(t->taps, 0, n * sizeof(float)));
+    return RZ_OK;
+}
+
+int rz_trainer_debug_tensor_dev(rz_trainer* t, int which, int layer, float* out, size_t n_floats, void* stream) {
+    RZ_REQUIRE(t && out, "rz_trainer_debug_tensor_dev: null pointer");
+    if (t->reps.size() > 1) { set_error("rz_trainer_debug_tensor_dev: not available on a data-parallel group"); return RZ_ESTATE; }
+    if (!t->last_batch) { set_error("rz_trainer_debug_tensor_dev: no step has run"); return RZ_ESTATE; }
+    const size_t B = t->last_batch, M = 64 * B, F = t->F, V = t->V, stride = 64 * t->act * F;
+    const bool tower = which == RZ_TRAIN_T_Y || which == RZ_TRAIN_T_A || which >= RZ_TRAIN_T_G;
+    const int layers = tower ? t->L : which == RZ_TRAIN_T_STATS ? t->L + 2 : 1;
+    RZ_REQUIRE(which >= 0 && which <= RZ_TRAIN_T_DZ, "rz_trainer_debug_tensor_dev: unknown tensor %d", which);
+    RZ_REQUIRE(layer >= 0 && layer < layers, "rz_trainer_debug_tensor_dev: layer %d outside [0, %d) for tensor %d", layer, layers, which);
+    RZ_REQUIRE(which != RZ_TRAIN_T_DZ || (layer >= 2 && layer % 2 == 0), "rz_trainer_debug_tensor_dev: layer %d keeps no dz", layer);
+    if (which >= RZ_TRAIN_T_G && !t->taps_valid) {
+        set_error("rz_trainer_debug_tensor_dev: the last step ran without rz_trainer_debug_keep_backward");
+        return RZ_ESTATE;
+    }
+    const float* src = nullptr;
+    size_t count = 0;
+    switch (which) {
+        case RZ_TRAIN_T_X0: src = t->x0; count = M * kCin0; break;
+        case RZ_TRAIN_T_Y: src = t->y + layer * stride; count = M * F; break;
+        case RZ_TRAIN_T_A: src = t->a + layer * stride; count = M * F; break;
+        case RZ_TRAIN_T_STATS: src = t->stats + (size_t)layer * 4 * F; count = 4 * F; break;
+        case RZ_TRAIN_T_STAT: src = t->stat; count = t->n; break;
+        case RZ_TRAIN_T_HC: src = t->hc; count = M * 3; break;
+        case RZ_TRAIN_T_AH: src = t->ah; count = M * 3; break;
+        case RZ_TRAIN_T_DH: src = t->dh; count = M * 3; break;
+        case RZ_TRAIN_T_DYH: src = t->dyh; count = M * 3; break;
+        case RZ_TRAIN_T_HP: src = t->hp; count = B * 128; break;
+        case RZ_TRAIN_T_HV: src = t->hv; count = B * 64; break;
+        case RZ_TRAIN_T_DL: src = t->dl; count = B * 64; break;
+        case RZ_TRAIN_T_H1: src = t->h1; count = B * V; break;
+        case RZ_TRAIN_T_DH1: src = t->dh1; count = B * V; break;
+        case RZ_TRAIN_T_DV: src = t->dv; count = B; break;
+        case RZ_TRAIN_T_LP: src = t->lp; count = B; break;
+        case RZ_TRAIN_T_LV: src = t->lv; count = B; break;
+        case RZ_TRAIN_T_LOSS_PV: src = t->loss_pv; count = 2; break;
+        default: src = t->taps + ((size_t)layer * 3 + (which - RZ_TRAIN_T_G)) * stride; count = M * F; break;  // G, DY, DZ
+    }
+    RZ_REQUIRE(n_floats == count, "rz_trainer_debug_tensor_dev: tensor %d has %zu floats, got %zu", which, count, n_floats);
+    RZ_CUDA_TRY(cudaSetDevice(t->device));
+    RZ_CUDA_TRY(cudaMemcpyAsync(out, src, count * sizeof(float), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+    return RZ_OK;
 }
 
 }  // extern "C"

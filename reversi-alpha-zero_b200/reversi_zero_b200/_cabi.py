@@ -129,6 +129,8 @@ SIGNATURES = {
     "rz_trainer_last_grad_dev": (C.c_int, [vp, vp, sz, vp]),
     "rz_trainer_replica_state_dev": (C.c_int, [vp, C.c_int, vp, vp, sz, vp]),
     "rz_trainer_debug_conv_dev": (C.c_int, [vp, C.c_int, vp, vp, vp, vp, sz, vp, vp]),
+    "rz_trainer_debug_tensor_dev": (C.c_int, [vp, C.c_int, C.c_int, vp, sz, vp]),
+    "rz_trainer_debug_keep_backward": (C.c_int, [vp, C.c_int]),
 }
 
 _lib = None

@@ -22,6 +22,9 @@ MOMENTUM = 0.9      # SGD(momentum=0.9), worker/optimize.py:84
 BN_MOMENTUM = 0.99  # Keras BatchNormalization default
 # ops of Trainer.debug_conv (RZ_TRAIN_CONV* in include/rz_engine.h)
 CONV0_FWD, CONV_FWD, CONV_DGRAD, CONV_WGRAD, CONV0_WGRAD = 0, 1, 2, 3, 4
+# tensors of Trainer.debug_tensor, in RZ_TRAIN_T_* order (include/rz_engine.h)
+DEBUG_TENSORS = ("x0", "y", "a", "stats", "stat", "hc", "ah", "dh", "dyh", "hp", "hv", "dl", "h1", "dh1", "dv", "lp", "lv",
+                 "loss_pv", "g", "dy", "dz")
 
 
 class Trainer:
@@ -37,6 +40,7 @@ class Trainer:
         self.mc = model_config
         self.devices = devices
         self.max_batch = int(max_batch)
+        self._last_batch = None
         self._h = C.c_void_p()
         ncfg = _cabi.NetCfg(model_config.cnn_filter_num, model_config.res_layer_num, model_config.value_fc_size,
                             model_config.cnn_filter_size)
@@ -94,6 +98,7 @@ class Trainer:
                                                      C.c_void_p(z.data_ptr()), n, C.c_void_p(index.data_ptr()), index.numel(),
                                                      float(lr), C.c_void_p(loss.data_ptr()), self._stream()),
                     "rz_trainer_step_dev")
+        self._last_batch = index.numel()
         return loss
 
     def last_grad(self):
@@ -127,6 +132,29 @@ class Trainer:
         ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
         _cabi.check(_cabi.lib().rz_trainer_debug_conv_dev(self._h, op, ptr(x), ptr(kernel), ptr(bias), ptr(add), batch, ptr(out),
                                                           self._stream()), "rz_trainer_debug_conv_dev")
+        return out
+
+    def debug_keep_backward(self, on):
+        """test hook (rz_trainer_debug_keep_backward, single trainers): make the following steps keep every tower layer's
+        backward tensors "g", "dy" and "dz" for debug_tensor"""
+        _cabi.check(_cabi.lib().rz_trainer_debug_keep_backward(self._h, int(bool(on))), "rz_trainer_debug_keep_backward")
+
+    def debug_tensor(self, name, layer=0):
+        """test hook (rz_trainer_debug_tensor_dev, single trainers): a new float32 CUDA tensor holding one intermediate
+        tensor of the last step, one of DEBUG_TENSORS, in its natural shape: [64 * B][16] for x0, [64 * B][F] for the
+        tower's y, a, g, dy, dz (``layer`` l), [4][F] for stats (slot ``layer``), [blob floats] for stat, [64 * B][3] for
+        hc, ah, dh, dyh, [B][128 | 64 | V] for hp, hv, dl, h1, dh1, [B] for dv, lp, lv and [2] for loss_pv."""
+        import torch
+        if self._last_batch is None:
+            raise RuntimeError("debug_tensor: no step has run")
+        F, V, B = self.mc.cnn_filter_num, self.mc.value_fc_size, self._last_batch
+        shape = {"x0": (64 * B, 16), "stats": (4, F), "stat": (self.blob_floats,), "hp": (B, 128), "hv": (B, 64), "dl": (B, 64),
+                 "h1": (B, V), "dh1": (B, V), "dv": (B,), "lp": (B,), "lv": (B,), "loss_pv": (2,)}.get(name)
+        if shape is None:
+            shape = (64 * B, 3) if name in ("hc", "ah", "dh", "dyh") else (64 * B, F)
+        out = torch.empty(shape, dtype=torch.float32, device=self.device)
+        _cabi.check(_cabi.lib().rz_trainer_debug_tensor_dev(self._h, DEBUG_TENSORS.index(name), layer, C.c_void_p(out.data_ptr()),
+                                                            out.numel(), self._stream()), "rz_trainer_debug_tensor_dev")
         return out
 
     def close(self):

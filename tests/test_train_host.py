@@ -118,6 +118,53 @@ def test_conv_gemm_restatement_matches_torch(batch, cin, cout):
               torch.nn.grad.conv2d_weight(x, kt.shape, dy, padding=1).permute(2, 3, 1, 0).reshape(9, cin, cout))
 
 
+@pytest.mark.parametrize("cfg,batch", [(MINI, 6), (dict(cnn_filter_num=48, res_layer_num=2, value_fc_size=24), 5)],
+                         ids=["mini", "48x2"])
+def test_stage_chain_matches_autograd(cfg, batch):
+    """oracle/train.py's per-stage references (the fp64 side of tests/test_train_stages_gpu.py), chained in the device
+    step's order and layout, give loss_and_grad's losses, batch statistics and every gradient to 1e-10 relative"""
+    mc = M.ModelConfig(**cfg)
+    w = _weights(mc, 8)
+    planes, policy, z = _batch(batch, 9)
+    policy[0] = np.eye(64)[17]   # a one-hot target
+    l2 = 1e-4
+    losses, grads, stats = ot.loss_and_grad(w, planes, policy, z, mc.res_layer_num, l2)
+    sl, sg, ss = ot.stage_loss_and_grad({k: torch.from_numpy(v) for k, v in w.items()}, planes, policy, z, mc.res_layer_num, l2)
+    for a, b in zip(sl, losses):
+        assert abs(a - b) <= 1e-10 * abs(b), (sl, losses)
+    rel = lambda a, b: np.linalg.norm(np.asarray(a, np.float64).ravel() - np.asarray(b).ravel()) / max(np.linalg.norm(b), 1e-300)
+    assert set(sg) == set(grads)
+    for name, g in grads.items():
+        if name.endswith(".bias") and not name.startswith(("policy_fc", "value_fc")):   # exactly 0 up to rounding in both
+            assert np.abs(sg[name].numpy()).max() < 1e-12 and np.abs(g).max() < 1e-12, name
+        else:
+            assert sg[name].shape == g.shape and rel(sg[name].numpy(), g) <= 1e-10, (name, rel(sg[name].numpy(), g))
+    assert set(ss) == set(stats)
+    for name, (m, v) in stats.items():
+        assert rel(ss[name][0].numpy(), m) <= 1e-10 and rel(ss[name][1].numpy(), v) <= 1e-10, name
+
+
+def test_stage_update_is_keras_sgd():
+    """the update stage: L2 on kernels only, Keras momentum form, moving averages"""
+    w, vel, g = (torch.tensor([0.5, -2.0], dtype=torch.float64), torch.tensor([0.1, 0.3], dtype=torch.float64),
+                 torch.tensor([1.0, -1.0], dtype=torch.float64))
+    nw, nv, ng = ot.sgd_update(w, vel, g, 0.1, 0.9, 1e-2, kernel=True)
+    assert torch.allclose(ng, torch.tensor([1.01, -1.04], dtype=torch.float64), rtol=0, atol=1e-15)
+    assert torch.allclose(nv, 0.9 * vel - 0.1 * ng, rtol=0, atol=1e-15) and torch.allclose(nw, w + nv, rtol=0, atol=1e-15)
+    assert torch.equal(ot.sgd_update(w, vel, g, 0.1, 0.9, 1e-2, kernel=False)[2], g)
+    assert ot.moving_average(2.0, 4.0, 0.99) == pytest.approx(2.02, rel=1e-15)
+
+
+DEBUG_SYMBOLS = ("rz_trainer_debug_tensor_dev", "rz_trainer_debug_keep_backward")
+
+
+def test_debug_tensor_symbols_resolve():
+    lib = C.CDLL(_cabi.LIB_PATH)
+    for name in DEBUG_SYMBOLS:
+        assert getattr(lib, name, None) is not None, name
+        assert name in _cabi.SIGNATURES
+
+
 @pytest.mark.parametrize("filters,res,kernel,batch", [(24, 1, 3, 8), (8, 1, 3, 8), (272, 1, 3, 8), (16, 1, 5, 8), (16, 1, 3, 0)])
 def test_trainer_rejects_unsupported_configurations(filters, res, kernel, batch):
     ncfg = _cabi.NetCfg(filters, res, 8, kernel)
