@@ -80,6 +80,29 @@ int rz_solve_dev(const uint64_t* own, const uint64_t* enemy, const uint8_t* exac
                  void* stream);
 int rz_solve(const uint64_t* own, const uint64_t* enemy, const uint8_t* exactly, int8_t* move, int8_t* score, size_t n);
 
+/* Deep exact endgame solver (csrc/rz_solver_deep.cu): the exact mode of rz_solve for positions with up to 30 empty
+ * squares, each solved by the whole current device (null-window probes over a split AND/OR tree, one lane per leaf).
+ * Host arrays; the n positions are solved one after another; synchronous.  For each position in the mover's frame:
+ * score[i] = exact final disc difference (empties not awarded), move[i] = first square in ascending order reaching it.
+ * move[i] = -1 and score[i] = 0 when the mover has no legal move (a finished game included), the position has more
+ * than 30 empties, or `timeout_s` seconds passed before the answer was proven (checked between slices, so a call
+ * returns within the timeout plus one slice plus the host's split time).  stats: nullable, n entries.
+ * Workspace: allocated on first use per device and kept (about 200 MB on a 132-SM H100); one call per device at a time. */
+typedef struct rz_deep_solve_stats {
+    int32_t probes;      /* null-window probes (value and move) */
+    int32_t slices;      /* kernel slices */
+    int32_t resplits;    /* open leaves the host split again between slices */
+    int32_t pad;
+    int64_t leaves;      /* leaves of the split trees, summed over probes */
+    int64_t node_steps;  /* node steps of the leaf machines */
+    double seconds;      /* wall time of the position */
+} rz_deep_solve_stats;
+int rz_solve_deep(const uint64_t* own, const uint64_t* enemy, int8_t* move, int8_t* score, size_t n, double timeout_s,
+                  rz_deep_solve_stats* stats);
+/* Tuning of rz_solve_deep for tests and measurements: slice length (us), leaf target of the split and leaf floor
+ * (empties below which the split stops); 0 restores each default (4000 us, one leaf per lane, 10 empties). */
+int rz_solve_deep_tune(int slice_us, int leaf_target, int leaf_floor);
+
 /* Scalar host twins for the single-environment Python objects (ReversiEnv / Board used by the
  * reference's evaluate.py, nboard.py, game_model.py): same header-only code as the device kernels
  * (csrc/rz_bitboard.cuh), compiled for the host.  Not a fallback for the batched path. */

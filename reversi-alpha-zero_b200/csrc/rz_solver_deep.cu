@@ -1,0 +1,506 @@
+// rz_solver_deep.cu -- exact endgame solver that puts the whole device on one position (rz_solve_deep, include/rz_engine.h).
+//
+// The value is found by null-window probes "value >= t?" (t = 1, then 0, then bisection: at most 8 probes over
+// [-64, 64]); the move by one more forest of probes over the root moves whose standing the value probes left open.
+// One probe is an AND/OR tree:
+//   * split: the host expands the probe root breadth-first in the lane solver's move order into a node table until the
+//     frontier holds `leaf_target` leaves or every leaf is down to `leaf_floor` empties.  A move flips the threshold to
+//     1 - t in the child's frame, a pass keeps side and threshold; finished games resolve when they are created;
+//   * leaves: a persistent kernel runs in slices of `slice_us`; every lane claims leaves in depth-first move order and runs
+//     the resumable null-window machine of rz_solver_deep.cuh on them, polling every kPollEvery node steps whether an
+//     ancestor has been decided meanwhile (then the leaf is dropped) or the slice is over (then its stack is parked);
+//   * resolution: a node is TRUE once one child proves it, FALSE once all children have failed to (a pending-children
+//     counter); each decision is one CAS on the status word and climbs until it meets an ancestor already decided;
+//   * between slices the host checks the timeout, and when fewer open leaves are left than lanes it re-splits the open
+//     leaves that have run longest into their children (dropping their parked stacks), so skewed subtrees spread out.
+// Booleans combine exactly, so the answer depends on nothing but the position (and on the timeout, only whether it hits).
+#include <algorithm>
+#include <chrono>
+#include <vector>
+
+#include "rz_common.cuh"
+#include "rz_solver_deep.cuh"
+
+namespace rz {
+namespace deep {
+
+constexpr int kBlockThreads = 128;
+constexpr int kBlocksPerSm = 4;
+constexpr int kPollEvery = 64;        // node steps between two abort / deadline checks of a leaf
+constexpr int kMaxNodes = 1 << 21;    // node table capacity per probe
+constexpr int kMaxRoots = 32;         // roots of a forest (one per root move)
+constexpr int kDefaultSliceUs = 4000;
+constexpr int kDefaultLeafFloor = 10;
+constexpr int kCtxPerLane = 2;        // parked stacks per lane
+
+enum : int32_t { kOpen = 0, kTrue = 1, kFalse = 2 };
+
+struct Node {  // 24 B, written by the host only
+    u64 own, enemy;
+    int32_t parent;  // -1: a root
+    int8_t t;        // the question: value(own to move) >= t ?
+    int8_t flip;     // 1: the node's answer is negated for its parent (opponent to move); 0: pass.  Roots: the wanted answer
+    int8_t empties;
+    int8_t leaf;
+};
+
+struct SliceArgs {
+    const Node* nodes;
+    int32_t* status;
+    int32_t* pending;
+    int32_t* ctx;              // parked stack of a leaf: slot index, -1 none
+    unsigned long long* steps; // node steps a leaf has run
+    const int32_t* claim;      // open leaves in depth-first order
+    int32_t n_claim;
+    int32_t* claim_next;
+    int32_t* stop;             // set when the roots answer the question
+    int32_t n_roots;
+    LeafFrame* ctx_frames;     // kLeafStack frames per slot
+    int32_t* ctx_depth;
+    const int32_t* free_slots;
+    int32_t n_free;
+    int32_t* free_next;
+    unsigned long long* total_steps;
+    long long slice_ns;
+};
+
+RZ_HD bool roots_answered(const volatile int32_t* status, const Node* nodes, int n_roots) {
+    // the lowest root whose answer is the wanted one, with every lower root decided the other way; or all decided
+    for (int i = 0; i < n_roots; ++i) {
+        const int s = status[i];
+        if (s == kOpen) return false;
+        if ((s == kTrue) == (nodes[i].flip != 0)) return true;
+    }
+    return true;
+}
+
+__device__ bool decided_above(const SliceArgs& a, int node) {
+    const volatile int32_t* st = a.status;
+    if (*(volatile int32_t*)a.stop) return true;
+    for (int c = node; c >= 0; c = a.nodes[c].parent)
+        if (st[c] != kOpen) return true;
+    return false;
+}
+
+__device__ void resolve(const SliceArgs& a, int node, bool r) {
+    int c = node;
+    while (true) {
+        if (atomicCAS(&a.status[c], kOpen, r ? kTrue : kFalse) != kOpen) return;
+        const int p = a.nodes[c].parent;
+        if (p < 0) {
+            __threadfence();
+            if (roots_answered(a.status, a.nodes, a.n_roots)) atomicExch(a.stop, 1);
+            return;
+        }
+        if (a.nodes[c].flip ? !r : r) { r = true; c = p; continue; }
+        if (atomicSub(&a.pending[p], 1) == 1) { r = false; c = p; continue; }
+        return;
+    }
+}
+
+__global__ void __launch_bounds__(kBlockThreads, kBlocksPerSm) deep_slice_kernel(SliceArgs a) {
+    LeafFrame stk[kLeafStack];
+    const long long deadline = solver::global_ns() + a.slice_ns;
+    unsigned long long lane_steps = 0;
+    while (true) {
+        if (*(volatile int32_t*)a.stop || solver::global_ns() > deadline) break;
+        const int i = atomicAdd(a.claim_next, 1);
+        if (i >= a.n_claim) break;
+        const int node = a.claim[i];
+        if (decided_above(a, node)) continue;
+        int depth;
+        const int slot = a.ctx[node];
+        if (slot >= 0) {
+            depth = a.ctx_depth[slot];
+            const LeafFrame* src = a.ctx_frames + (size_t)slot * kLeafStack;
+            for (int k = 0; k <= depth; ++k) stk[k] = src[k];
+        } else {
+            leaf_init(stk, depth, a.nodes[node].own, a.nodes[node].enemy, a.nodes[node].t);
+        }
+        long long steps = 0;
+        bool out_of_time = false;
+        const int r = leaf_advance(stk, depth, steps, kPollEvery, [&]() {
+            if (decided_above(a, node)) return false;
+            out_of_time = solver::global_ns() > deadline;
+            return !out_of_time;
+        });
+        atomicAdd(&a.steps[node], (unsigned long long)steps);
+        lane_steps += steps;
+        if (r != kLeafSuspended) { resolve(a, node, r == kLeafTrue); continue; }
+        if (!out_of_time) continue;  // an ancestor was decided: the leaf is moot
+        int s = slot;
+        if (s < 0) {
+            const int f = atomicAdd(a.free_next, 1);
+            s = f < a.n_free ? a.free_slots[f] : -1;
+        }
+        if (s >= 0) {  // park the stack; without a free slot the leaf starts over in a later slice
+            LeafFrame* dst = a.ctx_frames + (size_t)s * kLeafStack;
+            for (int k = 0; k <= depth; ++k) dst[k] = stk[k];
+            a.ctx_depth[s] = depth;
+        }
+        a.ctx[node] = s;
+        break;
+    }
+    atomicAdd(a.total_steps, lane_steps);
+}
+
+// ---------------------------------------------------------------------------------------------------------------- host
+
+struct Tuning {
+    int slice_us = 0, leaf_target = 0, leaf_floor = 0;  // 0: default
+};
+static Tuning g_tuning;
+
+struct Workspace {
+    int lanes = 0, ctx_slots = 0;
+    Node* nodes = nullptr;
+    int32_t *status = nullptr, *pending = nullptr, *ctx = nullptr, *claim = nullptr, *ctx_depth = nullptr, *free_slots = nullptr;
+    int32_t* counters = nullptr;  // claim_next, stop, free_next, pad
+    unsigned long long *steps = nullptr, *total_steps = nullptr;
+    LeafFrame* ctx_frames = nullptr;
+};
+
+// One probe forest on the host: the authoritative copy between slices.
+struct Tree {
+    std::vector<Node> nodes;
+    std::vector<int32_t> status, pending, ctx, first_child, n_children;
+    std::vector<unsigned long long> steps;
+    int n_roots = 0;
+    long long leaves = 0;
+
+    int add(u64 own, u64 enemy, int parent, int t, int flip) {
+        Node n;
+        n.own = own; n.enemy = enemy; n.parent = parent; n.t = (int8_t)t; n.flip = (int8_t)flip;
+        n.empties = (int8_t)(64 - popc64(own | enemy)); n.leaf = 1;
+        nodes.push_back(n);
+        status.push_back(kOpen); pending.push_back(0); ctx.push_back(-1); first_child.push_back(-1); n_children.push_back(0);
+        steps.push_back(0);
+        ++leaves;
+        return (int)nodes.size() - 1;
+    }
+    bool decided_above(int c) const {
+        for (; c >= 0; c = nodes[c].parent)
+            if (status[c] != kOpen) return true;
+        return false;
+    }
+    void resolve(int c, bool r) {  // resolve() of the kernel, sequential
+        while (true) {
+            if (status[c] != kOpen) return;
+            status[c] = r ? kTrue : kFalse;
+            const int p = nodes[c].parent;
+            if (p < 0) return;
+            if (nodes[c].flip ? !r : r) { r = true; c = p; continue; }
+            if (--pending[p] == 0) { r = false; c = p; continue; }
+            return;
+        }
+    }
+    bool answered() const { return roots_answered(status.data(), nodes.data(), n_roots); }
+    // Replace leaf i by its children in the lane solver's move order; finished games resolve at once.
+    void expand(int i) {
+        const Node n = nodes[i];
+        u64 moves = find_correct_moves(n.own, n.enemy);
+        const bool ordered = n.empties >= kOrderMinEmpties;
+        const int first = (int)nodes.size();
+        int count = 0;
+        int terminal_sq[32], terminal_r[32], n_terminal = 0;
+        nodes[i].leaf = 0; ctx[i] = -1; --leaves;
+        first_child[i] = first;
+        while (moves) {
+            const int a = solver::pick_move(n.own, n.enemy, moves, ordered);
+            moves &= ~(1ULL << a);
+            LeafFrame c;
+            int diff;
+            if (child_after(n.own, n.enemy, a, n.t, c, diff)) {
+                add(c.own, c.enemy, i, c.t, c.flip);
+            } else {  // game over: a node that is decided on creation (flip 0: its answer is the parent's)
+                const int k = add(0, 0, i, 0, 0);
+                nodes[k].leaf = 0; nodes[k].empties = 0; --leaves;
+                terminal_sq[n_terminal] = k; terminal_r[n_terminal++] = diff >= n.t;
+            }
+            ++count;
+        }
+        n_children[i] = count;
+        pending[i] = count;
+        for (int k = 0; k < n_terminal; ++k) resolve(terminal_sq[k], terminal_r[k] != 0);
+    }
+    // open leaves (no decided ancestor), depth first in move order
+    void open_leaves(std::vector<int32_t>& out) const {
+        out.clear();
+        std::vector<int> stack;
+        for (int r = n_roots - 1; r >= 0; --r) stack.push_back(r);
+        while (!stack.empty()) {
+            const int c = stack.back();
+            stack.pop_back();
+            if (status[c] != kOpen) continue;
+            if (nodes[c].leaf) { out.push_back(c); continue; }
+            for (int k = n_children[c] - 1; k >= 0; --k) stack.push_back(first_child[c] + k);
+        }
+    }
+};
+
+struct ProbeRun {
+    int slice_us, leaf_target, leaf_floor;
+    std::chrono::steady_clock::time_point deadline;
+    rz_deep_solve_stats* stats;
+};
+
+static int upload_and_run(Workspace& w, Tree& T, const std::vector<int32_t>& claim, const std::vector<int32_t>& free_slots,
+                          int slice_us) {
+    const size_t n = T.nodes.size();
+    RZ_CUDA_TRY(cudaMemcpy(w.nodes, T.nodes.data(), n * sizeof(Node), cudaMemcpyHostToDevice));
+    RZ_CUDA_TRY(cudaMemcpy(w.status, T.status.data(), n * 4, cudaMemcpyHostToDevice));
+    RZ_CUDA_TRY(cudaMemcpy(w.pending, T.pending.data(), n * 4, cudaMemcpyHostToDevice));
+    RZ_CUDA_TRY(cudaMemcpy(w.ctx, T.ctx.data(), n * 4, cudaMemcpyHostToDevice));
+    RZ_CUDA_TRY(cudaMemcpy(w.steps, T.steps.data(), n * 8, cudaMemcpyHostToDevice));
+    RZ_CUDA_TRY(cudaMemcpy(w.claim, claim.data(), claim.size() * 4, cudaMemcpyHostToDevice));
+    if (!free_slots.empty())
+        RZ_CUDA_TRY(cudaMemcpy(w.free_slots, free_slots.data(), free_slots.size() * 4, cudaMemcpyHostToDevice));
+    RZ_CUDA_TRY(cudaMemset(w.counters, 0, 4 * sizeof(int32_t)));
+    SliceArgs a;
+    a.nodes = w.nodes; a.status = w.status; a.pending = w.pending; a.ctx = w.ctx; a.steps = w.steps;
+    a.claim = w.claim; a.n_claim = (int32_t)claim.size(); a.claim_next = w.counters; a.stop = w.counters + 1;
+    a.n_roots = T.n_roots; a.ctx_frames = w.ctx_frames; a.ctx_depth = w.ctx_depth;
+    a.free_slots = w.free_slots; a.n_free = (int32_t)free_slots.size(); a.free_next = w.counters + 2;
+    a.total_steps = w.total_steps; a.slice_ns = (long long)slice_us * 1000;
+    deep_slice_kernel<<<(unsigned)(w.lanes / kBlockThreads), kBlockThreads>>>(a);
+    RZ_LAUNCH_CHECK();
+    RZ_CUDA_TRY(cudaMemcpy(T.status.data(), w.status, n * 4, cudaMemcpyDeviceToHost));
+    RZ_CUDA_TRY(cudaMemcpy(T.pending.data(), w.pending, n * 4, cudaMemcpyDeviceToHost));
+    RZ_CUDA_TRY(cudaMemcpy(T.ctx.data(), w.ctx, n * 4, cudaMemcpyDeviceToHost));
+    RZ_CUDA_TRY(cudaMemcpy(T.steps.data(), w.steps, n * 8, cudaMemcpyDeviceToHost));
+    return RZ_OK;
+}
+
+// Decide the roots of T as far as the forest's question needs.  *timed_out is set when the deadline passed first.
+static int run_forest(Workspace& w, Tree& T, const ProbeRun& P, bool* timed_out) {
+    *timed_out = false;
+    // split breadth-first, one level at a time, down to the leaf target or the leaf floor
+    std::vector<int32_t> level, claim, free_slots;
+    T.open_leaves(level);
+    while (!T.answered() && T.leaves < P.leaf_target) {
+        if (std::chrono::steady_clock::now() > P.deadline) { *timed_out = true; return RZ_OK; }
+        bool grew = false;
+        for (int c : level) {
+            if (T.leaves >= P.leaf_target || T.nodes.size() + 64 > (size_t)kMaxNodes) break;
+            if (T.decided_above(c) || T.nodes[c].empties <= P.leaf_floor) continue;
+            T.expand(c);
+            grew = true;
+        }
+        if (!grew) break;
+        T.open_leaves(level);
+    }
+    std::vector<int> order;
+    std::vector<char> used(w.ctx_slots);
+    while (!T.answered()) {
+        if (std::chrono::steady_clock::now() > P.deadline) { *timed_out = true; return RZ_OK; }
+        T.open_leaves(claim);
+        if ((int)claim.size() < w.lanes) {  // lanes would sit idle: re-split the longest-running open leaves
+            order.clear();
+            for (int c : claim)
+                if (T.nodes[c].empties > P.leaf_floor && T.steps[c] > 0) order.push_back(c);
+            std::stable_sort(order.begin(), order.end(), [&](int x, int y) { return T.steps[x] > T.steps[y]; });
+            long long open = (long long)claim.size();
+            int split = 0;
+            for (int c : order) {
+                if (open >= w.lanes || T.nodes.size() + 64 > (size_t)kMaxNodes) break;
+                if (T.decided_above(c)) continue;
+                const long long before = T.leaves;
+                T.expand(c);
+                open += T.leaves - before;
+                ++split;
+            }
+            if (split) {
+                if (P.stats) P.stats->resplits += split;
+                if (T.answered()) break;
+                T.open_leaves(claim);
+            }
+        }
+        RZ_REQUIRE(!claim.empty(), "rz_solve_deep: undecided roots without an open leaf");
+        std::fill(used.begin(), used.end(), 0);
+        for (int c : claim)
+            if (T.ctx[c] >= 0) used[T.ctx[c]] = 1;
+        free_slots.clear();
+        for (int s = 0; s < w.ctx_slots; ++s)
+            if (!used[s]) free_slots.push_back(s);
+        RZ_TRY(upload_and_run(w, T, claim, free_slots, P.slice_us));
+        if (P.stats) P.stats->slices += 1;
+    }
+    return RZ_OK;
+}
+
+static int workspace(Workspace** out) {
+    constexpr int kMaxDevices = 64;
+    static Workspace* ws[kMaxDevices] = {};
+    int dev = 0;
+    RZ_CUDA_TRY(cudaGetDevice(&dev));
+    RZ_REQUIRE(dev >= 0 && dev < kMaxDevices, "rz_solve_deep: device index out of range");
+    if (!ws[dev]) {
+        Workspace* w = new Workspace;
+        w->lanes = num_sms() * kBlocksPerSm * kBlockThreads;
+        w->ctx_slots = w->lanes * kCtxPerLane;
+        RZ_CUDA_TRY(cudaMalloc((void**)&w->nodes, (size_t)kMaxNodes * sizeof(Node)));
+        RZ_CUDA_TRY(cudaMalloc((void**)&w->status, (size_t)kMaxNodes * 4));
+        RZ_CUDA_TRY(cudaMalloc((void**)&w->pending, (size_t)kMaxNodes * 4));
+        RZ_CUDA_TRY(cudaMalloc((void**)&w->ctx, (size_t)kMaxNodes * 4));
+        RZ_CUDA_TRY(cudaMalloc((void**)&w->claim, (size_t)kMaxNodes * 4));
+        RZ_CUDA_TRY(cudaMalloc((void**)&w->steps, (size_t)kMaxNodes * 8));
+        RZ_CUDA_TRY(cudaMalloc((void**)&w->ctx_depth, (size_t)w->ctx_slots * 4));
+        RZ_CUDA_TRY(cudaMalloc((void**)&w->free_slots, (size_t)w->ctx_slots * 4));
+        RZ_CUDA_TRY(cudaMalloc((void**)&w->ctx_frames, (size_t)w->ctx_slots * kLeafStack * sizeof(LeafFrame)));
+        RZ_CUDA_TRY(cudaMalloc((void**)&w->counters, 4 * sizeof(int32_t)));
+        RZ_CUDA_TRY(cudaMalloc((void**)&w->total_steps, sizeof(unsigned long long)));
+        ws[dev] = w;
+    }
+    *out = ws[dev];
+    return RZ_OK;
+}
+
+// Bounds on the value of each root move, in the root mover's frame, learned from decided root children.
+struct MoveBounds {
+    int lo[64], hi[64];
+};
+
+static void learn_root_children(const Tree& T, int root, MoveBounds& B, const int* child_sq) {
+    if (T.first_child[root] < 0) return;
+    for (int k = 0; k < T.n_children[root]; ++k) {
+        const int c = T.first_child[root] + k;
+        const int s = T.status[c];
+        if (s == kOpen) continue;
+        const int sq = child_sq[k];
+        // the child's answer r to "value_c >= t_c"; flip: the move's value is -value_c, else value_c
+        const Node& n = T.nodes[c];
+        const bool r = s == kTrue;
+        if (n.empties == 0 && !n.leaf && n.own == 0 && n.enemy == 0) continue;  // a finished game: known exactly already
+        if (n.flip) {
+            if (r) B.hi[sq] = std::min(B.hi[sq], -n.t); else B.lo[sq] = std::max(B.lo[sq], 1 - n.t);
+        } else {
+            if (r) B.lo[sq] = std::max(B.lo[sq], (int)n.t); else B.hi[sq] = std::min(B.hi[sq], n.t - 1);
+        }
+    }
+}
+
+static int solve_one(Workspace& w, u64 own, u64 enemy, int8_t* move_out, int8_t* score_out, const ProbeRun& P) {
+    *move_out = -1; *score_out = 0;
+    const u64 legal = find_correct_moves(own, enemy);
+    if (!legal || 64 - popc64(own | enemy) > kDeepMaxEmpties) return RZ_OK;
+    // root moves in the split's order, and their exact values where the game ends
+    int child_sq[32], n_moves = 0;
+    MoveBounds B;
+    for (int s = 0; s < 64; ++s) { B.lo[s] = -64; B.hi[s] = 64; }
+    {
+        u64 m = legal;
+        const bool ordered = 64 - popc64(own | enemy) >= kOrderMinEmpties;
+        while (m) {
+            const int a = solver::pick_move(own, enemy, m, ordered);
+            m &= ~(1ULL << a);
+            child_sq[n_moves++] = a;
+            LeafFrame c;
+            int diff;
+            if (!child_after(own, enemy, a, 0, c, diff)) B.lo[a] = B.hi[a] = diff;
+        }
+    }
+    Tree T;
+    bool timed_out = false;
+    auto probe = [&](int t, bool* r) -> int {
+        T = Tree();
+        T.n_roots = 1;
+        T.add(own, enemy, -1, t, 0);
+        if (P.stats) P.stats->probes += 1;
+        RZ_TRY(run_forest(w, T, P, &timed_out));
+        if (P.stats) P.stats->leaves += T.leaves;
+        *r = T.status[0] == kTrue;
+        learn_root_children(T, 0, B, child_sq);
+        return RZ_OK;
+    };
+    // value: t = 1, t = 0, then bisection inside the known sign range
+    int lo = -64, hi = 64;
+    bool r;
+    RZ_TRY(probe(1, &r));
+    if (timed_out) return RZ_OK;
+    if (r) lo = 1; else hi = 0;
+    if (!r) {
+        RZ_TRY(probe(0, &r));
+        if (timed_out) return RZ_OK;
+        if (r) lo = 0; else hi = -1;
+    }
+    while (lo < hi) {
+        const int mid = lo + (hi - lo + 1) / 2;
+        RZ_TRY(probe(mid, &r));
+        if (timed_out) return RZ_OK;
+        if (r) lo = mid; else hi = mid - 1;
+    }
+    const int v = lo;
+    // move: the first square whose move reaches v.  Squares already known to fall short are skipped; the open ones below
+    // the first known best move are probed together, one root each ("does this move reach v?")
+    int known_best = 64;
+    for (int s = 0; s < 64; ++s)
+        if ((legal >> s & 1) && B.lo[s] >= v) { known_best = s; break; }
+    int open_sq[kMaxRoots], n_open = 0;
+    for (int s = 0; s < known_best; ++s)
+        if ((legal >> s & 1) && B.hi[s] >= v) open_sq[n_open++] = s;
+    int best = known_best;
+    if (n_open) {
+        T = Tree();
+        for (int k = 0; k < n_open; ++k) {
+            LeafFrame c;
+            int diff;
+            child_after(own, enemy, open_sq[k], v, c, diff);  // never a finished game: those are known exactly
+            // opponent to move: the move reaches v iff NOT (value_c >= 1 - v); pass: iff value_c >= v.  `flip` of a
+            // root holds the wanted answer.
+            T.add(c.own, c.enemy, -1, c.t, c.flip ? 0 : 1);
+        }
+        T.n_roots = n_open;
+        if (P.stats) P.stats->probes += 1;
+        RZ_TRY(run_forest(w, T, P, &timed_out));
+        if (timed_out) return RZ_OK;
+        if (P.stats) P.stats->leaves += T.leaves;
+        for (int k = 0; k < n_open; ++k)
+            if ((T.status[k] == kTrue) == (T.nodes[k].flip != 0)) { best = open_sq[k]; break; }
+    }
+    if (best >= 64) return RZ_OK;  // cannot happen: some move reaches the value
+    *move_out = (int8_t)best; *score_out = (int8_t)v;
+    return RZ_OK;
+}
+
+}  // namespace deep
+}  // namespace rz
+
+using namespace rz;
+
+extern "C" {
+
+int rz_solve_deep_tune(int slice_us, int leaf_target, int leaf_floor) {
+    RZ_REQUIRE(slice_us >= 0 && leaf_target >= 0 && leaf_floor >= 0, "rz_solve_deep_tune: negative argument");
+    deep::g_tuning.slice_us = slice_us;
+    deep::g_tuning.leaf_target = leaf_target;
+    deep::g_tuning.leaf_floor = leaf_floor;
+    return RZ_OK;
+}
+
+int rz_solve_deep(const uint64_t* own, const uint64_t* enemy, int8_t* move, int8_t* score, size_t n, double timeout_s,
+                  rz_deep_solve_stats* stats) {
+    RZ_REQUIRE(n == 0 || (own && enemy && move && score), "rz_solve_deep: null pointer");
+    deep::Workspace* w = nullptr;
+    if (n) RZ_TRY(deep::workspace(&w));
+    for (size_t i = 0; i < n; ++i) {
+        const auto t0 = std::chrono::steady_clock::now();
+        deep::ProbeRun P;
+        P.slice_us = deep::g_tuning.slice_us ? deep::g_tuning.slice_us : deep::kDefaultSliceUs;
+        P.leaf_target = deep::g_tuning.leaf_target ? deep::g_tuning.leaf_target : w->lanes;
+        P.leaf_floor = deep::g_tuning.leaf_floor ? deep::g_tuning.leaf_floor : deep::kDefaultLeafFloor;
+        P.deadline = t0 + std::chrono::duration_cast<std::chrono::steady_clock::duration>(std::chrono::duration<double>(timeout_s));
+        P.stats = stats ? stats + i : nullptr;
+        if (P.stats) *P.stats = rz_deep_solve_stats{};
+        unsigned long long steps0 = 0, steps1 = 0;
+        if (P.stats) RZ_CUDA_TRY(cudaMemcpy(&steps0, w->total_steps, 8, cudaMemcpyDeviceToHost));
+        RZ_TRY(deep::solve_one(*w, own[i], enemy[i], move + i, score + i, P));
+        if (P.stats) {
+            RZ_CUDA_TRY(cudaMemcpy(&steps1, w->total_steps, 8, cudaMemcpyDeviceToHost));
+            P.stats->node_steps = (int64_t)(steps1 - steps0);
+            P.stats->seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+        }
+    }
+    return RZ_OK;
+}
+
+}  // extern "C"

@@ -58,6 +58,11 @@ class PlayRow(C.Structure):
     _fields_ = [("own", C.c_uint64), ("enemy", C.c_uint64), ("n_visit", C.c_int32 * 64), ("z", C.c_int32), ("pad", C.c_int32)]
 
 
+class DeepSolveStats(C.Structure):
+    _fields_ = [("probes", C.c_int32), ("slices", C.c_int32), ("resplits", C.c_int32), ("pad", C.c_int32),
+                ("leaves", C.c_int64), ("node_steps", C.c_int64), ("seconds", C.c_double)]
+
+
 class Stats(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in ("games_started", "games_finished", "expansions", "simulations", "waves",
                                           "plies", "nn_launches", "mcts_launches", "max_nodes_used", "max_edges_used")] + [
@@ -79,6 +84,8 @@ SIGNATURES = {
     "rz_dihedral_dev": (C.c_int, [vp, vp, vp, sz, vp]),
     "rz_solve_dev": (C.c_int, [vp, vp, vp, vp, vp, sz, vp]),
     "rz_solve": (C.c_int, [u64p, u64p, u8p, i8p, i8p, sz]),
+    "rz_solve_deep": (C.c_int, [u64p, u64p, i8p, i8p, sz, C.c_double, C.POINTER(DeepSolveStats)]),
+    "rz_solve_deep_tune": (C.c_int, [C.c_int, C.c_int, C.c_int]),
     "rz_find_correct_moves_host": (C.c_uint64, [C.c_uint64, C.c_uint64]),
     "rz_calc_flip_host": (C.c_uint64, [C.c_int, C.c_uint64, C.c_uint64]),
     "rz_dihedral_host": (C.c_uint64, [C.c_uint64, C.c_int]),

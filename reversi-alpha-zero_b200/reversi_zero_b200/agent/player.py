@@ -27,6 +27,11 @@ ActionWithEvaluation = namedtuple("ActionWithEvaluation", "action n q")
 logger = getLogger(__name__)
 
 
+def solver_max_empties(config):
+    """b200.solver_max_empties of a config; 12 (the lane solver alone) for a reference ``Config`` without ``b200``"""
+    return int(getattr(getattr(config, "b200", None), "solver_max_empties", 12))
+
+
 class ReversiPlayer:
     def __init__(self, config, model, play_config=None, enable_resign=True, mtcs_info=None, api=None, seed=0, device=0):
         """model: a ``reversi_zero_b200.net.Net`` (None selects the deterministic test evaluator).
@@ -95,8 +100,8 @@ class ReversiPlayer:
         self.requested_stop_thinking = False
         if pc.use_solver_turn and turn >= pc.use_solver_turn:  # action_by_searching, agent/player.py:100-103,150-161
             if self.solver is None:
-                from ..lib.reversi_solver import ReversiSolver
-                self.solver = ReversiSolver()
+                from ..lib import reversi_solver
+                self.solver = reversi_solver.ReversiSolver(solver_max_empties(self.config))
             mv, score = self.solver.solve(own, enemy, 1, exactly=True)
             if mv is not None:
                 policy = np.zeros(64)

@@ -132,6 +132,7 @@ class B200Config(_Section):
         self.write_play_rows = False  # also write play_*.rzrows (280 B per ply) for the device-side ingest, worker/ingest.py
         self.train_from_json = False  # opt: parse play_*.json itself on the device and ignore the rows twins (worker/optimize.py)
         self.train_devices = None   # opt: CUDA ordinals of a data-parallel training group, e.g. [0, 1]; None = the one device
+        self.solver_max_empties = 12  # ReversiPlayer's exact root solver: 13..this many empties go to the whole-GPU solver
 
 
 class Config(_Section):

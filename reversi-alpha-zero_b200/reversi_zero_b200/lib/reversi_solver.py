@@ -1,9 +1,14 @@
 """Mirror of the reference's ``ReversiSolver`` (lib/alt/reversi_solver_cython.pyx:32-61, imported by
-agent/player.py:15) over the device solver (csrc/rz_solver.cuh): ``solve(black, white, next_player, timeout,
-exactly) -> (move, score)`` or ``(None, None)``.  ``solve_batch`` solves many positions in one launch."""
+agent/player.py:15) over the device solvers: ``solve(black, white, next_player, timeout, exactly) -> (move, score)`` or
+``(None, None)``.  ``solve_batch`` solves many positions in one launch of the lane solver (csrc/rz_solver.cuh, up to 12
+empties); ``solve_deep_batch`` solves exact positions up to 30 empties one after another, each with the whole device
+(csrc/rz_solver_deep.cu)."""
 import numpy as np
 
 from .. import _cabi
+
+LANE_MAX_EMPTIES = 12   # the lane solver refuses larger positions
+DEEP_MAX_EMPTIES = 30   # ... and the deep solver
 
 
 def solve_batch(own, enemy, exactly):
@@ -18,13 +23,48 @@ def solve_batch(own, enemy, exactly):
     return move, score
 
 
+def solve_deep_batch(own, enemy, timeout=30.0, stats=False):
+    """Exact solve of each position (uint64 arrays in the mover's frame) with the whole device, one after another;
+    `timeout` seconds per position.  -> (move int8[], score int8[]) with move -1 = no legal move, more than 30 empties or
+    timed out; with stats=True also a list of dicts (probes, slices, resplits, leaves, node_steps, seconds)."""
+    own = np.ascontiguousarray(own, dtype=np.uint64).reshape(-1)
+    enemy = np.ascontiguousarray(enemy, dtype=np.uint64).reshape(-1)
+    move = np.empty(own.shape, np.int8)
+    score = np.empty(own.shape, np.int8)
+    st = (_cabi.DeepSolveStats * max(1, own.size))()
+    _cabi.check(_cabi.lib().rz_solve_deep(own.ctypes.data_as(_cabi.u64p), enemy.ctypes.data_as(_cabi.u64p),
+                                           move.ctypes.data_as(_cabi.i8p), score.ctypes.data_as(_cabi.i8p), own.size,
+                                           float(timeout), st), "rz_solve_deep")
+    if not stats:
+        return move, score
+    names = [f for f, _ in _cabi.DeepSolveStats._fields_ if f != "pad"]
+    return move, score, [{k: getattr(st[i], k) for k in names} for i in range(own.size)]
+
+
+def tune_deep(slice_us=0, leaf_target=0, leaf_floor=0):
+    """Slice length (us), split leaf target and leaf floor (empties) of the deep solver; 0 restores a default."""
+    _cabi.check(_cabi.lib().rz_solve_deep_tune(int(slice_us), int(leaf_target), int(leaf_floor)), "rz_solve_deep_tune")
+
+
 class ReversiSolver:
+    def __init__(self, max_empties=LANE_MAX_EMPTIES):
+        """max_empties: exact requests with 13..max_empties empty squares go to the deep solver with the caller's
+        timeout; at the default 12 every request goes to the lane solver, which refuses larger positions."""
+        if not LANE_MAX_EMPTIES <= int(max_empties) <= DEEP_MAX_EMPTIES:
+            raise ValueError(f"max_empties must be in {LANE_MAX_EMPTIES}..{DEEP_MAX_EMPTIES}, got {max_empties}")
+        self.max_empties = int(max_empties)
+
     def solve(self, black, white, next_player, timeout=30, exactly=False):
-        """next_player: Player enum (or its value: 1 black, 2 white).  `timeout` is accepted for compatibility; the device
-        solver refuses positions with more than 12 empty squares instead (returns (None, None) like a timeout)."""
+        """next_player: Player enum (or its value: 1 black, 2 white).  The lane solver refuses positions with more than
+        12 empty squares and ignores `timeout`; the deep solver (exact requests up to `max_empties`) gives up after
+        `timeout` seconds.  Both answer a refusal or a timeout with (None, None), like the reference's timeout."""
         p = getattr(next_player, "value", next_player)
         own, enemy = (black, white) if p == 1 else (white, black)
-        mv, sc = solve_batch([own], [enemy], [exactly])
+        empties = 64 - bin(int(own) | int(enemy)).count("1")
+        if exactly and LANE_MAX_EMPTIES < empties <= self.max_empties:
+            mv, sc = solve_deep_batch([own], [enemy], timeout)
+        else:
+            mv, sc = solve_batch([own], [enemy], [exactly])
         if mv[0] < 0:
             return None, None
         return int(mv[0]), int(sc[0])
