@@ -231,6 +231,12 @@ typedef struct rz_engine_cfg {
     int32_t arena_simulation_num;   /* the largest simulation count rz_engine_set_simulation_num will be asked for during this
                                        engine's life (the maximum over schedule_of_simulation_num_per_move and .force-sim,
                                        worker/self_play.py:262-272); the arenas are sized for it.  0 = simulation_num_per_move. */
+    int32_t eval_cache_mb;          /* device memory (MiB) of the evaluation cache: a leaf whose transformed board the network
+                                       evaluated before (in any game, with the weights now loaded) takes that result instead of
+                                       a tower row -- the same bits, so the games do not change.  0 = the environment variable
+                                       RZ_EVAL_CACHE_MB if set (read by rz_engine_create), else 2048; < 0 = off.  Always off
+                                       with RZ_EVAL_FAKE and while a second network is set.  Loading new weights into the
+                                       engine's network invalidates every entry. */
     float c_puct;                   /* :135 */
     float noise_eps;                /* :136 */
     float dirichlet_alpha;          /* :137 */
@@ -286,6 +292,11 @@ typedef struct rz_stats {
     uint64_t max_nodes_used, max_edges_used;
     double nn_ms, mcts_ms; /* device time (CUDA events on the engine's stream) spent in the two kernel families */
     double run_ms;         /* device time from the first to the last wave of each rz_engine_run call, accumulated */
+    uint64_t tower_rows;    /* leaves the evaluator ran (expansions counts every evaluated leaf, cache hits included) */
+    uint64_t cache_lookups; /* leaves looked up in the evaluation cache */
+    uint64_t cache_hits;    /* ... served from it (hit counts of a two-group engine depend on timing; results do not) */
+    uint64_t cache_repeats; /* tower rows not stored because their board was already in the cache when the wave's rows were
+                               inserted: boards that two leaves of the same wave sent to the tower */
 } rz_stats;
 
 int rz_engine_create(const rz_engine_cfg* cfg, rz_net* net /* may be NULL for RZ_EVAL_FAKE */, int device,
@@ -301,6 +312,10 @@ int rz_engine_run(rz_engine* e, uint64_t finished_target, uint64_t max_waves);
 int rz_engine_poll(rz_engine* e, rz_game* games, size_t game_cap, size_t* n_games, rz_ply* plies, size_t ply_cap,
                    size_t* n_plies);
 int rz_engine_stats(rz_engine* e, rz_stats* out);
+/* the cache_lookups / cache_hits of rz_stats split by the turn of the searched root: n must be 61; entry t < 60 counts
+ * searches at turn t, entry 60 every search of the first game of a slot of a warm_start engine (random pre-played
+ * openings, which rarely repeat). */
+int rz_engine_cache_turn_stats(rz_engine* e, uint64_t* lookups, uint64_t* hits, int n);
 /* no slot starts a game whose local index (slot + games already started by the slot x games) is >= max_games; 0 = no
  * limit, 1 = let the resident games finish and start nothing (rz_engine_run then returns when every slot is idle). */
 int rz_engine_set_max_games(rz_engine* e, uint64_t max_games);

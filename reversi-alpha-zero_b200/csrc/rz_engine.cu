@@ -124,11 +124,15 @@ struct Slot {
     uint32_t n_solves, n_searched_plies;
 };
 
+constexpr int kCacheTurnBuckets = 61;  // turns 0..59 of the searched root; 60: the warm-started first game of a slot
+
 struct Status {
     unsigned long long games_started, games_finished, expansions, simulations, plies, idle_slots;
     unsigned long long max_nodes, max_edges;
     int error;  // 0 or RZ_E*
     int pad;
+    unsigned long long tower_rows, cache_repeats;
+    unsigned long long cache_lookups[kCacheTurnBuckets], cache_hits[kCacheTurnBuckets];
 };
 
 struct DevCfg {
@@ -140,6 +144,14 @@ struct DevCfg {
     float warm_cdf[60];  // warm_start: P(first game of a slot begins at turn <= t), rz_engine_set_warm_start_profile
     float warm_waves[60];  // ... and the waves a search at turn t takes in a long-running engine (0 = unknown)
 };
+
+__device__ __forceinline__ uint32_t hash_key(u64 own, u64 enemy, uint32_t kpid) {
+    u64 h = own * 0x9E3779B97F4A7C15ULL ^ (enemy + 0x7F4A7C15ULL) * 0xC2B2AE3D27D4EB4FULL ^ (u64)kpid * 0x165667B19E3779F9ULL;
+    h ^= h >> 29; h *= 0xBF58476D1CE4E5B9ULL; h ^= h >> 32;
+    return (uint32_t)h;
+}
+
+#include "rz_eval_cache.cuh"
 
 struct DevPtrs {
     Slot* slots;
@@ -161,16 +173,11 @@ struct DevPtrs {
     solver::SolveCtx* sctx;  // [G][K + 1]
     uint32_t* sactive;       // [2 groups][2 parities][G * (K + 1)]
     uint32_t* solve_count;   // [2 groups][2 parities] (64 words apart)
-    float* keep_policy;      // [G*K][64]
+    float* keep_policy;      // [G*K][64]  (also where a leaf served by the evaluation cache finds its result)
     float* keep_value;       // [G*K]
     u64* solver_tt;          // per-lane transposition tables of the solver kernel, one set per slot group
+    EvalCache cache;         // evaluation cache shared by both slot groups (n_sets == 0: off)
 };
-
-__device__ __forceinline__ uint32_t hash_key(u64 own, u64 enemy, uint32_t kpid) {
-    u64 h = own * 0x9E3779B97F4A7C15ULL ^ (enemy + 0x7F4A7C15ULL) * 0xC2B2AE3D27D4EB4FULL ^ (u64)kpid * 0x165667B19E3779F9ULL;
-    h ^= h >> 29; h *= 0xBF58476D1CE4E5B9ULL; h ^= h >> 32;
-    return (uint32_t)h;
-}
 
 #include "rz_engine_warp.cuh"
 
@@ -265,7 +272,10 @@ struct rz_engine {
     cudaEvent_t ev_run[3];     // run start, run end, group-1 join
     int ev_used;
     double nn_ms, mcts_ms, run_ms;
+    uint32_t cache_sets;  // sets of the evaluation cache (0: off); dp.cache.n_sets is 0 while two networks play
 };
+
+constexpr int64_t kDefaultEvalCacheMb = 2048;
 
 static int collect_timing(rz_engine* e) {  // call after the stream has been synchronised
     for (int g = 0; g < e->n_groups; ++g)
@@ -321,6 +331,7 @@ static int drain_mailboxes(rz_engine* e) {
 static int launch_wave(rz_engine* e) {
     const DevCfg& c = e->dc;
     const bool timed = e->ev_used < 8;
+    if (e->dp.cache.n_sets) e->dp.cache.gen = (uint32_t)e->net->weights_version;  // new weights: every older entry misses
     for (int g = 0; g < e->n_groups; ++g) {
         cudaStream_t st = g == 0 ? e->stream : e->stream2;
         const int s0 = e->group_slot0[g], s1 = e->group_slot0[g + 1];
@@ -360,6 +371,13 @@ static int launch_wave(rz_engine* e) {
             }
         }
         if (timed) RZ_CUDA_TRY(cudaEventRecord(ev[2], st));
+        if (e->dp.cache.n_sets) {  // this wave's tower rows into the evaluation cache (outside the timed evaluation)
+            cache_insert_kernel<<<num_sms() * 2, 256, 0, st>>>(e->dp.cache, e->dp.batch_own + (size_t)s0 * c.K, e->dp.batch_enemy + (size_t)s0 * c.K,
+                                                              e->dp.policy + (size_t)s0 * c.K * 64, e->dp.value + (size_t)s0 * c.K,
+                                                              e->dp.batch_count + g * 64, &e->dp.status->cache_repeats);
+            RZ_LAUNCH_CHECK();
+            e->mcts_launches++;
+        }
     }
     if (timed) e->ev_used++;
     e->waves++;
@@ -402,6 +420,7 @@ int rz_engine_create(const rz_engine_cfg* cfg, rz_net* net, int device, rz_engin
     e->waves = e->nn_launches = e->mcts_launches = e->finished_total = 0;
     e->h_status = nullptr; e->h_flags = nullptr; e->stream = nullptr; e->stream2 = nullptr;
     e->ev_used = 0; e->nn_ms = e->mcts_ms = e->run_ms = 0.0;
+    e->cache_sets = 0;
     for (int i = 0; i < 48; ++i) e->ev[i] = nullptr;
     e->ev_run[0] = e->ev_run[1] = e->ev_run[2] = nullptr;
     // two slot groups on two streams: the MCTS tick of one group can run while the network launch of the other is in flight,
@@ -458,6 +477,22 @@ int rz_engine_create(const rz_engine_cfg* cfg, rz_net* net, int device, rz_engin
     if (!rc) rc = dev_alloc(e, (void**)&p.value, (B + 2) * sizeof(float), true);
     const bool solving = c.solver_turn > 0 || c.solver_sim_turn > 0;
     const size_t SR = G * (c.K + 1);
+    // evaluation cache: on by default for the network evaluator (RZ_EVAL_CACHE_MB overrides the default size)
+    int64_t cache_mb = cfg->eval_cache_mb;
+    if (cache_mb == 0) {
+        const char* env = getenv("RZ_EVAL_CACHE_MB");
+        cache_mb = env ? atoll(env) : kDefaultEvalCacheMb;
+    }
+    if (cfg->eval_mode != RZ_EVAL_NET) cache_mb = 0;
+    const size_t cache_sets = cache_mb > 0 ? (size_t)cache_mb * 1048576 / (kCacheWays * sizeof(EvalCacheEntry)) : 0;
+    p.cache.entries = nullptr; p.cache.next = nullptr; p.cache.n_sets = 0; p.cache.gen = 0;
+    if (!rc && cache_sets >= 0xFFFFFFFFull / kCacheWays) { set_error("eval_cache_mb too large (%lld)", (long long)cache_mb); rc = RZ_EINVAL; }
+    if (!rc && cache_sets) {
+        if (!rc) rc = dev_alloc(e, (void**)&p.cache.entries, cache_sets * kCacheWays * sizeof(EvalCacheEntry), true);
+        if (!rc) rc = dev_alloc(e, (void**)&p.cache.next, cache_sets * sizeof(uint32_t), true);
+        e->cache_sets = (uint32_t)cache_sets;
+        p.cache.n_sets = e->cache_sets;
+    }
     if (!rc) rc = dev_alloc(e, (void**)&p.solve_count, 1024, true);
     p.sctx = nullptr; p.sactive = nullptr; p.keep_policy = nullptr; p.keep_value = nullptr; p.solver_tt = nullptr;
     e->solve_parity[0] = e->solve_parity[1] = 0;
@@ -471,9 +506,11 @@ int rz_engine_create(const rz_engine_cfg* cfg, rz_net* net, int device, rz_engin
     if (solving) {
         if (!rc) rc = dev_alloc(e, (void**)&p.sctx, SR * sizeof(solver::SolveCtx), true);
         if (!rc) rc = dev_alloc(e, (void**)&p.sactive, 4 * SR * sizeof(uint32_t), true);
+        if (!rc) rc = dev_alloc(e, (void**)&p.solver_tt, e->solver_tt_words_per_group * 2 * sizeof(u64), true);
+    }
+    if (solving || cache_sets) {
         if (!rc) rc = dev_alloc(e, (void**)&p.keep_policy, G * c.K * 64 * sizeof(float), true);
         if (!rc) rc = dev_alloc(e, (void**)&p.keep_value, G * c.K * sizeof(float), true);
-        if (!rc) rc = dev_alloc(e, (void**)&p.solver_tt, e->solver_tt_words_per_group * 2 * sizeof(u64), true);
     }
     if (!rc && cudaMallocHost((void**)&e->h_status, sizeof(Status)) != cudaSuccess) { set_error("cudaMallocHost failed"); rc = RZ_ENOMEM; }
     if (!rc && cudaMallocHost((void**)&e->h_flags, G * 2) != cudaSuccess) { set_error("cudaMallocHost failed"); rc = RZ_ENOMEM; }
@@ -571,6 +608,19 @@ int rz_engine_stats(rz_engine* e, rz_stats* out) {
     out->mcts_launches = e->mcts_launches; out->max_nodes_used = s.max_nodes; out->max_edges_used = s.max_edges;
     RZ_TRY(collect_timing(e));
     out->nn_ms = e->nn_ms; out->mcts_ms = e->mcts_ms; out->run_ms = e->run_ms;
+    out->tower_rows = s.tower_rows; out->cache_repeats = s.cache_repeats;
+    out->cache_lookups = out->cache_hits = 0;
+    for (int b = 0; b < kCacheTurnBuckets; ++b) { out->cache_lookups += s.cache_lookups[b]; out->cache_hits += s.cache_hits[b]; }
+    return RZ_OK;
+}
+
+int rz_engine_cache_turn_stats(rz_engine* e, uint64_t* lookups, uint64_t* hits, int n) {
+    RZ_REQUIRE(e && lookups && hits && n == kCacheTurnBuckets, "rz_engine_cache_turn_stats: bad argument");
+    RZ_CUDA_TRY(cudaSetDevice(e->device));
+    RZ_TRY(sync_all(e));
+    RZ_CUDA_TRY(cudaMemcpyAsync(e->h_status, e->dp.status, sizeof(Status), cudaMemcpyDeviceToHost, e->stream));
+    RZ_CUDA_TRY(cudaStreamSynchronize(e->stream));
+    for (int b = 0; b < n; ++b) { lookups[b] = e->h_status->cache_lookups[b]; hits[b] = e->h_status->cache_hits[b]; }
     return RZ_OK;
 }
 
@@ -616,6 +666,7 @@ int rz_engine_set_second_net(rz_engine* e, rz_net* net_b, int enable) {
     RZ_REQUIRE(e->waves == 0, "rz_engine_set_second_net: must be called before the first wave");
     e->net_b = enable ? net_b : nullptr;
     e->dc.two_nets = enable ? 1 : 0;
+    e->dp.cache.n_sets = enable ? 0u : e->cache_sets;  // a leaf's result then depends on which network is to move
     return RZ_OK;
 }
 

@@ -684,8 +684,30 @@ __global__ void __launch_bounds__(kWarpTickThreads) tick_warp_kernel(const DevCf
     // 3. gather: network leaves (K3: dihedral-transformed bitboards) and solver requests go to their own compact batches
     const bool mine = lane < n_leaves;
     const bool is_solve = mine && x.desc[sl.pending[mine ? lane : 0]].dihedral == kSolveMarker;
-    const unsigned sv_mask = __ballot_sync(0xffffffffu, is_solve), nn_mask = __ballot_sync(0xffffffffu, mine && !is_solve);
+    const bool is_leaf = mine && !is_solve;
+    u64 t_own = 0, t_enemy = 0;
+    bool hit = false;
+    if (is_leaf) {
+        const Descent& d = x.desc[sl.pending[lane]];
+        t_own = dihedral(d.leaf_own, d.dihedral);
+        t_enemy = dihedral(d.leaf_enemy, d.dihedral);
+        if (p.cache.n_sets) {  // a hit goes to the descent's keep row, which consume() reads when `kept` is set
+            const size_t row = (size_t)s * c.K + sl.pending[lane];
+            hit = cache_lookup(p.cache, t_own, t_enemy, p.keep_policy + row * 64, p.keep_value + row);
+        }
+    }
+    const unsigned sv_mask = __ballot_sync(0xffffffffu, is_solve), nn_mask = __ballot_sync(0xffffffffu, is_leaf && !hit);
     const uint32_t n_nn = __popc(nn_mask), n_sv = __popc(sv_mask) + root_req;
+    const uint32_t n_hit = __popc(__ballot_sync(0xffffffffu, hit));
+    if (lane == 0 && n_nn + n_hit > 0) {
+        if (p.cache.n_sets) {
+            const int turn = popc64(sl.root_own | sl.root_enemy) - 4;
+            const int b = (c.warm_start && sl.games_played == 1) ? kCacheTurnBuckets - 1 : (turn < 0 ? 0 : (turn > 59 ? 59 : turn));
+            atomicAdd(&p.status->cache_lookups[b], (unsigned long long)(n_nn + n_hit));
+            if (n_hit) atomicAdd(&p.status->cache_hits[b], (unsigned long long)n_hit);
+        }
+        if (n_nn) atomicAdd(&p.status->tower_rows, (unsigned long long)n_nn);
+    }
     const uint32_t net = c.two_nets ? sl.cur_net : 0u;  // evaluation matches: every search is evaluated by the mover's network
     uint32_t base = 0, sbase = 0;
     uint32_t* s_count = p.solve_count + (group * 2 + parity) * 64;
@@ -697,13 +719,15 @@ __global__ void __launch_bounds__(kWarpTickThreads) tick_warp_kernel(const DevCf
     if (root_req) sl.root_req = 0;
     x.write_back();
     const uint32_t below = (1u << lane) - 1u;
-    if (mine && !is_solve) {
+    if (hit) {
+        x.desc[sl.pending[lane]].kept = 1;
+    } else if (is_leaf) {
         Descent& d = x.desc[sl.pending[lane]];
         const uint32_t at = net * (uint32_t)c.G * (uint32_t)c.K + (uint32_t)slot0 * (uint32_t)c.K + base + __popc(nn_mask & below);
         d.leaf_index = at;
         d.kept = 0;
-        p.batch_own[at] = dihedral(d.leaf_own, d.dihedral);
-        p.batch_enemy[at] = dihedral(d.leaf_enemy, d.dihedral);
+        p.batch_own[at] = t_own;
+        p.batch_enemy[at] = t_enemy;
     } else if (is_solve) {  // WLD solve of a simulation's position: context of this descent
         const int di = sl.pending[lane];
         const Descent& d = x.desc[di];

@@ -235,6 +235,7 @@ static int finish_load(rz_net* net, cudaStream_t stream) {
     else if (tc_width(F)) RZ_TRY(net_pack_tc_narrow(net, stream));
     RZ_CUDA_TRY(cudaStreamSynchronize(stream));
     net->loaded = true;
+    net->weights_version++;
     return RZ_OK;
 }
 

@@ -15,6 +15,7 @@ struct rz_net {
     rz_net_cfg cfg;
     int device;
     bool loaded;
+    uint64_t weights_version;  // 1, 2, ...: counts the weight loads (tags the engine's evaluation cache entries)
     size_t blob_floats;
     float* blob;         // device copy of the fp32 blob (Keras layouts), used by the generic kernel and the heads
     float* scale_shift;  // [n_conv_layers][2][F] folded BN of conv0 + tower convs; then heads: [2][2] policy, [2][1] value

@@ -36,7 +36,7 @@ class EngineCfg(C.Structure):
         "games", "simulation_num_per_move", "parallel_search_num", "virtual_loss", "change_tau_turn", "thinking_loop",
         "required_visit_to_decide_action", "start_rethinking_turn", "allowed_resign_turn", "use_resign_threshold",
         "share_mtcs_info", "eval_mode", "net_impl", "max_plies", "warm_start", "overlap_groups", "max_sims_per_wave", "use_solver_turn", "use_solver_turn_in_simulation",
-        "reset_mtcs_info_per_game", "max_searches_per_game", "arena_simulation_num")] + [(n, C.c_float) for n in (
+        "reset_mtcs_info_per_game", "max_searches_per_game", "arena_simulation_num", "eval_cache_mb")] + [(n, C.c_float) for n in (
             "c_puct", "noise_eps", "dirichlet_alpha", "resign_threshold", "disable_resignation_rate")] + [
         (n, C.c_uint64) for n in ("seed", "first_game_id", "game_id_stride", "max_games")]
 
@@ -66,7 +66,8 @@ class DeepSolveStats(C.Structure):
 class Stats(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in ("games_started", "games_finished", "expansions", "simulations", "waves",
                                           "plies", "nn_launches", "mcts_launches", "max_nodes_used", "max_edges_used")] + [
-        ("nn_ms", C.c_double), ("mcts_ms", C.c_double), ("run_ms", C.c_double)]
+        ("nn_ms", C.c_double), ("mcts_ms", C.c_double), ("run_ms", C.c_double)] + [
+        (n, C.c_uint64) for n in ("tower_rows", "cache_lookups", "cache_hits", "cache_repeats")]
 
 
 # name -> (restype, argtypes); every symbol include/rz_engine.h declares
@@ -110,6 +111,7 @@ SIGNATURES = {
     "rz_engine_run": (C.c_int, [vp, C.c_uint64, C.c_uint64]),
     "rz_engine_poll": (C.c_int, [vp, C.POINTER(Game), sz, C.POINTER(sz), C.POINTER(Ply), sz, C.POINTER(sz)]),
     "rz_engine_stats": (C.c_int, [vp, C.POINTER(Stats)]),
+    "rz_engine_cache_turn_stats": (C.c_int, [vp, u64p, u64p, C.c_int]),
     "rz_engine_set_simulation_num": (C.c_int, [vp, C.c_int32]),
     "rz_engine_set_warm_start_profile": (C.c_int, [vp, f32p, C.c_int]),
     "rz_engine_set_max_games": (C.c_int, [vp, C.c_uint64]),

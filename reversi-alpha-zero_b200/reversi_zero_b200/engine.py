@@ -11,9 +11,9 @@ EVAL_NET, EVAL_FAKE = 0, 1
 
 def engine_cfg_from_play_config(pc, pdc=None, games=1024, seed=0, eval_mode=EVAL_NET, net_impl=0, first_game_id=0,
                                 game_id_stride=1, max_games=0, warm_start=False, overlap_groups=0,
-                                max_searches_per_game=0, use_solver=True, arena_simulation_num=0):
+                                max_searches_per_game=0, use_solver=True, arena_simulation_num=0, eval_cache_mb=0):
     """Build an rz_engine_cfg from objects with the reference's PlayConfig / PlayDataConfig fields
-    (config.py:116-166)."""
+    (config.py:116-166).  eval_cache_mb: size of the evaluation cache (0 = default, < 0 = off; include/rz_engine.h)."""
     cfg = _cabi.EngineCfg()
     cfg.games = games
     cfg.simulation_num_per_move = int(pc.simulation_num_per_move)
@@ -33,6 +33,7 @@ def engine_cfg_from_play_config(pc, pdc=None, games=1024, seed=0, eval_mode=EVAL
     cfg.overlap_groups = overlap_groups
     cfg.max_searches_per_game = max_searches_per_game
     cfg.arena_simulation_num = int(arena_simulation_num or 0)
+    cfg.eval_cache_mb = int(eval_cache_mb)
     cfg.max_sims_per_wave = int(getattr(pc, "max_sims_per_wave", 0) or 0)
     cfg.reset_mtcs_info_per_game = int(getattr(pc, "reset_mtcs_info_per_game", 1) or 1) if cfg.share_mtcs_info else 1
     cfg.use_solver_turn = int(getattr(pc, "use_solver_turn", 0) or 0) if use_solver else 0
@@ -94,6 +95,14 @@ class Engine:
         s = _cabi.Stats()
         _cabi.check(_cabi.lib().rz_engine_stats(self._h, C.byref(s)), "rz_engine_stats")
         return {n: (float if t is C.c_double else int)(getattr(s, n)) for n, t in _cabi.Stats._fields_}
+
+    def cache_turn_stats(self):
+        """-> (lookups, hits): numpy uint64 [61]; entry t < 60 counts searches at turn t, entry 60 the warm-started first
+        games of the slots (rz_engine_cache_turn_stats)."""
+        lookups, hits = np.zeros(61, np.uint64), np.zeros(61, np.uint64)
+        _cabi.check(_cabi.lib().rz_engine_cache_turn_stats(self._h, lookups.ctypes.data_as(_cabi.u64p), hits.ctypes.data_as(_cabi.u64p), 61),
+                    "rz_engine_cache_turn_stats")
+        return lookups, hits
 
     def set_simulation_num(self, sims):
         _cabi.check(_cabi.lib().rz_engine_set_simulation_num(self._h, int(sims)), "rz_engine_set_simulation_num")
