@@ -87,7 +87,10 @@ int rz_solve(const uint64_t* own, const uint64_t* enemy, const uint8_t* exactly,
  * move[i] = -1 and score[i] = 0 when the mover has no legal move (a finished game included), the position has more
  * than 30 empties, or `timeout_s` seconds passed before the answer was proven (checked between slices, so a call
  * returns within the timeout plus one slice plus the host's split time).  stats: nullable, n entries.
- * Workspace: allocated on first use per device and kept (about 200 MB on a 132-SM H100); one call per device at a time. */
+ * Workspace: allocated on first use per device and kept (about 1.3 GB on a 132-SM H100: 240 MB of node table and parked
+ * stacks, and the 1 GiB transposition table); one call per device at a time.  The transposition table holds proven
+ * bounds only, shared by the probes of a call and kept across calls, so consecutive positions of one game reuse each
+ * other's proofs; it changes the work, never an answer. */
 typedef struct rz_deep_solve_stats {
     int32_t probes;      /* null-window probes (value and move) */
     int32_t slices;      /* kernel slices */
@@ -100,8 +103,28 @@ typedef struct rz_deep_solve_stats {
 int rz_solve_deep(const uint64_t* own, const uint64_t* enemy, int8_t* move, int8_t* score, size_t n, double timeout_s,
                   rz_deep_solve_stats* stats);
 /* Tuning of rz_solve_deep for tests and measurements: slice length (us), leaf target of the split and leaf floor
- * (empties below which the split stops); 0 restores each default (4000 us, one leaf per lane, 10 empties). */
+ * (empties below which the split stops); 0 restores each default (4000 us, one leaf per lane, 10 empties).  The next
+ * call starts from an empty transposition table, so that it searches under the new tuning. */
 int rz_solve_deep_tune(int slice_us, int leaf_target, int leaf_floor);
+/* The deep solver's transposition table on the current device, for tests and measurements.  rz_solve_deep_table sets its
+ * size (rounded down to a power of two of 128-byte buckets, at least one; 0 restores the default 1 GiB) from the next
+ * rz_solve_deep call on, which then starts from an empty table, as after rz_solve_deep_tune.  rz_solve_deep_clear
+ * empties the table and zeroes its counts now.  rz_solve_deep_table_stats: counts since the table was last emptied
+ * (all zero before the first call). */
+typedef struct rz_deep_table_stats {
+    int64_t lookups;   /* frames looked up before they were searched */
+    int64_t cutoffs;   /* ... decided by a stored bound, without search */
+    int64_t hints;     /* ... that tried the stored best move first */
+    int64_t stores;    /* decided frames written to a new entry */
+    int64_t replaced;  /* ... of those, over another position's entry */
+    int64_t merges;    /* decided frames merged into their position's entry */
+    int64_t dropped;   /* stores dropped because another writer held the entry */
+    int64_t occupied;  /* entries holding a position now */
+    int64_t bytes;     /* table size */
+} rz_deep_table_stats;
+int rz_solve_deep_table(int64_t bytes);
+int rz_solve_deep_clear(void);
+int rz_solve_deep_table_stats(rz_deep_table_stats* out);
 
 /* Scalar host twins for the single-environment Python objects (ReversiEnv / Board used by the
  * reference's evaluate.py, nboard.py, game_model.py): same header-only code as the device kernels

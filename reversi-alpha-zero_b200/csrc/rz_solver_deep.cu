@@ -12,7 +12,10 @@
 //   * resolution: a node is TRUE once one child proves it, FALSE once all children have failed to (a pending-children
 //     counter); each decision is one CAS on the status word and climbs until it meets an ancestor already decided;
 //   * between slices the host checks the timeout, and when fewer open leaves are left than lanes it re-splits the open
-//     leaves that have run longest into their children (dropping their parked stacks), so skewed subtrees spread out.
+//     leaves that have run longest into their children (dropping their parked stacks), so skewed subtrees spread out;
+//   * the transposition table (rz_solver_deep.cuh) is shared by every lane and kept across probes and calls: the leaf
+//     machines look up the frames they enter and store the frames they decide, and resolve() stores the split-tree nodes
+//     it decides, which are the largest subtrees and the first ones the next probe revisits.
 // Booleans combine exactly, so the answer depends on nothing but the position (and on the timeout, only whether it hits).
 #include <algorithm>
 #include <chrono>
@@ -32,6 +35,7 @@ constexpr int kMaxRoots = 32;         // roots of a forest (one per root move)
 constexpr int kDefaultSliceUs = 4000;
 constexpr int kDefaultLeafFloor = 10;
 constexpr int kCtxPerLane = 2;        // parked stacks per lane
+constexpr long long kDefaultTableBytes = 1LL << 30;
 
 enum : int32_t { kOpen = 0, kTrue = 1, kFalse = 2 };
 
@@ -62,6 +66,8 @@ struct SliceArgs {
     int32_t* free_next;
     unsigned long long* total_steps;
     long long slice_ns;
+    Table table;
+    unsigned long long* table_counts;  // kTabCounters
 };
 
 RZ_HD bool roots_answered(const volatile int32_t* status, const Node* nodes, int n_roots) {
@@ -82,18 +88,25 @@ __device__ bool decided_above(const SliceArgs& a, int node) {
     return false;
 }
 
-__device__ void resolve(const SliceArgs& a, int node, bool r) {
-    int c = node;
+// The leaf `node` is decided r: climb while it decides ancestors, storing each ancestor it decides in the table (the
+// leaf's own answer is stored by its machine, or came from the table).
+__device__ void resolve(const SliceArgs& a, int node, bool r, TableLane& tl) {
+    int c = node, from = -1;  // from: the child whose answer decided c
     while (true) {
         if (atomicCAS(&a.status[c], kOpen, r ? kTrue : kFalse) != kOpen) return;
-        const int p = a.nodes[c].parent;
+        const Node& n = a.nodes[c];
+        if (from >= 0) {  // TRUE: the proving move is the square the child has and c has not
+            const u64 placed = (a.nodes[from].own | a.nodes[from].enemy) & ~(n.own | n.enemy);
+            tl.store(n.own, n.enemy, n.t, r, r && placed ? ctz64(placed) : -1);
+        }
+        const int p = n.parent;
         if (p < 0) {
             __threadfence();
             if (roots_answered(a.status, a.nodes, a.n_roots)) atomicExch(a.stop, 1);
             return;
         }
-        if (a.nodes[c].flip ? !r : r) { r = true; c = p; continue; }
-        if (atomicSub(&a.pending[p], 1) == 1) { r = false; c = p; continue; }
+        if (n.flip ? !r : r) { r = true; from = c; c = p; continue; }
+        if (atomicSub(&a.pending[p], 1) == 1) { r = false; from = c; c = p; continue; }
         return;
     }
 }
@@ -102,6 +115,9 @@ __global__ void __launch_bounds__(kBlockThreads, kBlocksPerSm) deep_slice_kernel
     LeafFrame stk[kLeafStack];
     const long long deadline = solver::global_ns() + a.slice_ns;
     unsigned long long lane_steps = 0;
+    TableLane tl;
+    tl.tab = a.table;
+    for (int k = 0; k < kTabCounters; ++k) tl.cnt[k] = 0;
     while (true) {
         if (*(volatile int32_t*)a.stop || solver::global_ns() > deadline) break;
         const int i = atomicAdd(a.claim_next, 1);
@@ -116,17 +132,19 @@ __global__ void __launch_bounds__(kBlockThreads, kBlocksPerSm) deep_slice_kernel
             for (int k = 0; k <= depth; ++k) stk[k] = src[k];
         } else {
             leaf_init(stk, depth, a.nodes[node].own, a.nodes[node].enemy, a.nodes[node].t);
+            const int known = tl.enter(stk[0]);  // a stored bound may decide the leaf at once
+            if (known >= 0) { resolve(a, node, known != 0, tl); continue; }
         }
         long long steps = 0;
         bool out_of_time = false;
-        const int r = leaf_advance(stk, depth, steps, kPollEvery, [&]() {
+        const int r = leaf_advance(stk, depth, steps, kPollEvery, tl, [&]() {
             if (decided_above(a, node)) return false;
             out_of_time = solver::global_ns() > deadline;
             return !out_of_time;
         });
         atomicAdd(&a.steps[node], (unsigned long long)steps);
         lane_steps += steps;
-        if (r != kLeafSuspended) { resolve(a, node, r == kLeafTrue); continue; }
+        if (r != kLeafSuspended) { resolve(a, node, r == kLeafTrue, tl); continue; }
         if (!out_of_time) continue;  // an ancestor was decided: the leaf is moot
         int s = slot;
         if (s < 0) {
@@ -142,12 +160,27 @@ __global__ void __launch_bounds__(kBlockThreads, kBlocksPerSm) deep_slice_kernel
         break;
     }
     atomicAdd(a.total_steps, lane_steps);
+    for (int k = 0; k < kTabCounters; ++k) {  // every lane of the grid's full warps gets here
+        const unsigned v = __reduce_add_sync(0xffffffffu, tl.cnt[k]);
+        if ((threadIdx.x & 31) == 0 && v) atomicAdd(a.table_counts + k, (unsigned long long)v);
+    }
+}
+
+// Occupied entries of the table into *out.
+__global__ void table_count_kernel(const TableEntry* e, size_t n, unsigned long long* out) {
+    unsigned c = 0;
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+        c += (e[i].own | e[i].enemy) != 0;
+    c = __reduce_add_sync(0xffffffffu, c);
+    if ((threadIdx.x & 31) == 0 && c) atomicAdd(out, (unsigned long long)c);
 }
 
 // ---------------------------------------------------------------------------------------------------------------- host
 
 struct Tuning {
     int slice_us = 0, leaf_target = 0, leaf_floor = 0;  // 0: default
+    long long table_bytes = 0;
+    int generation = 0;  // counts the calls of rz_solve_deep_tune / rz_solve_deep_table
 };
 static Tuning g_tuning;
 
@@ -158,6 +191,10 @@ struct Workspace {
     int32_t* counters = nullptr;  // claim_next, stop, free_next, pad
     unsigned long long *steps = nullptr, *total_steps = nullptr;
     LeafFrame* ctx_frames = nullptr;
+    Table table{nullptr, 0};
+    size_t table_entries = 0;
+    int table_generation = -1;  // the tuning the table was emptied for
+    unsigned long long* table_counts = nullptr;  // kTabCounters, then the occupied count of rz_solve_deep_table_stats
 };
 
 // One probe forest on the host: the authoritative copy between slices.
@@ -262,6 +299,7 @@ static int upload_and_run(Workspace& w, Tree& T, const std::vector<int32_t>& cla
     a.n_roots = T.n_roots; a.ctx_frames = w.ctx_frames; a.ctx_depth = w.ctx_depth;
     a.free_slots = w.free_slots; a.n_free = (int32_t)free_slots.size(); a.free_next = w.counters + 2;
     a.total_steps = w.total_steps; a.slice_ns = (long long)slice_us * 1000;
+    a.table = w.table; a.table_counts = w.table_counts;
     deep_slice_kernel<<<(unsigned)(w.lanes / kBlockThreads), kBlockThreads>>>(a);
     RZ_LAUNCH_CHECK();
     RZ_CUDA_TRY(cudaMemcpy(T.status.data(), w.status, n * 4, cudaMemcpyDeviceToHost));
@@ -328,13 +366,43 @@ static int run_forest(Workspace& w, Tree& T, const ProbeRun& P, bool* timed_out)
     return RZ_OK;
 }
 
+constexpr int kMaxDevices = 64;
+static Workspace* g_ws[kMaxDevices] = {};
+
+static int current_device(int* dev) {
+    RZ_CUDA_TRY(cudaGetDevice(dev));
+    RZ_REQUIRE(*dev >= 0 && *dev < kMaxDevices, "rz_solve_deep: device index out of range");
+    return RZ_OK;
+}
+
+static int clear_table(Workspace& w) {
+    RZ_CUDA_TRY(cudaMemset(w.table.entries, 0, w.table_entries * sizeof(TableEntry)));
+    RZ_CUDA_TRY(cudaMemset(w.table_counts, 0, (kTabCounters + 1) * sizeof(unsigned long long)));
+    return RZ_OK;
+}
+
+// After a tuning call, an empty table of the size rz_solve_deep_table asked for (the largest power of two of buckets that
+// fits), so that a test or measurement under the new tuning searches instead of answering from earlier proofs.
+static int prepare_table(Workspace& w) {
+    if (w.table_generation == g_tuning.generation) return RZ_OK;
+    const long long bytes = g_tuning.table_bytes ? g_tuning.table_bytes : kDefaultTableBytes;
+    u64 buckets = 1;
+    while ((long long)(buckets * 2 * kTableWays * sizeof(TableEntry)) <= bytes) buckets *= 2;
+    if (!w.table.entries || w.table.mask + 1 != buckets) {
+        if (w.table.entries) RZ_CUDA_TRY(cudaFree(w.table.entries));
+        w.table.entries = nullptr;
+        w.table_entries = (size_t)buckets * kTableWays;
+        RZ_CUDA_TRY(cudaMalloc((void**)&w.table.entries, w.table_entries * sizeof(TableEntry)));
+        w.table.mask = buckets - 1;
+    }
+    w.table_generation = g_tuning.generation;
+    return clear_table(w);
+}
+
 static int workspace(Workspace** out) {
-    constexpr int kMaxDevices = 64;
-    static Workspace* ws[kMaxDevices] = {};
     int dev = 0;
-    RZ_CUDA_TRY(cudaGetDevice(&dev));
-    RZ_REQUIRE(dev >= 0 && dev < kMaxDevices, "rz_solve_deep: device index out of range");
-    if (!ws[dev]) {
+    RZ_TRY(current_device(&dev));
+    if (!g_ws[dev]) {
         Workspace* w = new Workspace;
         w->lanes = num_sms() * kBlocksPerSm * kBlockThreads;
         w->ctx_slots = w->lanes * kCtxPerLane;
@@ -349,9 +417,11 @@ static int workspace(Workspace** out) {
         RZ_CUDA_TRY(cudaMalloc((void**)&w->ctx_frames, (size_t)w->ctx_slots * kLeafStack * sizeof(LeafFrame)));
         RZ_CUDA_TRY(cudaMalloc((void**)&w->counters, 4 * sizeof(int32_t)));
         RZ_CUDA_TRY(cudaMalloc((void**)&w->total_steps, sizeof(unsigned long long)));
-        ws[dev] = w;
+        RZ_CUDA_TRY(cudaMalloc((void**)&w->table_counts, (kTabCounters + 1) * sizeof(unsigned long long)));
+        g_ws[dev] = w;
     }
-    *out = ws[dev];
+    RZ_TRY(prepare_table(*g_ws[dev]));
+    *out = g_ws[dev];
     return RZ_OK;
 }
 
@@ -474,6 +544,46 @@ int rz_solve_deep_tune(int slice_us, int leaf_target, int leaf_floor) {
     deep::g_tuning.slice_us = slice_us;
     deep::g_tuning.leaf_target = leaf_target;
     deep::g_tuning.leaf_floor = leaf_floor;
+    ++deep::g_tuning.generation;
+    return RZ_OK;
+}
+
+int rz_solve_deep_table(int64_t bytes) {
+    RZ_REQUIRE(bytes >= 0, "rz_solve_deep_table: negative size");
+    deep::g_tuning.table_bytes = bytes;
+    ++deep::g_tuning.generation;
+    return RZ_OK;
+}
+
+int rz_solve_deep_clear(void) {
+    int dev = 0;
+    RZ_TRY(deep::current_device(&dev));
+    if (deep::g_ws[dev]) RZ_TRY(deep::clear_table(*deep::g_ws[dev]));
+    return RZ_OK;
+}
+
+int rz_solve_deep_table_stats(rz_deep_table_stats* out) {
+    RZ_REQUIRE(out, "rz_solve_deep_table_stats: null pointer");
+    *out = rz_deep_table_stats{};
+    int dev = 0;
+    RZ_TRY(deep::current_device(&dev));
+    deep::Workspace* w = deep::g_ws[dev];
+    if (!w) return RZ_OK;
+    unsigned long long* occupied = w->table_counts + deep::kTabCounters;
+    RZ_CUDA_TRY(cudaMemset(occupied, 0, sizeof(unsigned long long)));
+    deep::table_count_kernel<<<(unsigned)num_sms() * 8, 256>>>(w->table.entries, w->table_entries, occupied);
+    RZ_LAUNCH_CHECK();
+    unsigned long long c[deep::kTabCounters + 1];
+    RZ_CUDA_TRY(cudaMemcpy(c, w->table_counts, sizeof(c), cudaMemcpyDeviceToHost));
+    out->lookups = (int64_t)c[deep::kTabLookups];
+    out->cutoffs = (int64_t)c[deep::kTabCutoffs];
+    out->hints = (int64_t)c[deep::kTabHints];
+    out->stores = (int64_t)c[deep::kTabStores];
+    out->replaced = (int64_t)c[deep::kTabReplaced];
+    out->merges = (int64_t)c[deep::kTabMerges];
+    out->dropped = (int64_t)c[deep::kTabDropped];
+    out->occupied = (int64_t)c[deep::kTabCounters];
+    out->bytes = (int64_t)(w->table_entries * sizeof(deep::TableEntry));
     return RZ_OK;
 }
 

@@ -63,6 +63,11 @@ class DeepSolveStats(C.Structure):
                 ("leaves", C.c_int64), ("node_steps", C.c_int64), ("seconds", C.c_double)]
 
 
+class DeepTableStats(C.Structure):
+    _fields_ = [(n, C.c_int64) for n in ("lookups", "cutoffs", "hints", "stores", "replaced", "merges", "dropped",
+                                         "occupied", "bytes")]
+
+
 class Stats(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in ("games_started", "games_finished", "expansions", "simulations", "waves",
                                           "plies", "nn_launches", "mcts_launches", "max_nodes_used", "max_edges_used")] + [
@@ -87,6 +92,9 @@ SIGNATURES = {
     "rz_solve": (C.c_int, [u64p, u64p, u8p, i8p, i8p, sz]),
     "rz_solve_deep": (C.c_int, [u64p, u64p, i8p, i8p, sz, C.c_double, C.POINTER(DeepSolveStats)]),
     "rz_solve_deep_tune": (C.c_int, [C.c_int, C.c_int, C.c_int]),
+    "rz_solve_deep_table": (C.c_int, [C.c_int64]),
+    "rz_solve_deep_clear": (C.c_int, []),
+    "rz_solve_deep_table_stats": (C.c_int, [C.POINTER(DeepTableStats)]),
     "rz_find_correct_moves_host": (C.c_uint64, [C.c_uint64, C.c_uint64]),
     "rz_calc_flip_host": (C.c_uint64, [C.c_int, C.c_uint64, C.c_uint64]),
     "rz_dihedral_host": (C.c_uint64, [C.c_uint64, C.c_int]),

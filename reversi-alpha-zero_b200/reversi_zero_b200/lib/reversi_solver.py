@@ -2,7 +2,9 @@
 agent/player.py:15) over the device solvers: ``solve(black, white, next_player, timeout, exactly) -> (move, score)`` or
 ``(None, None)``.  ``solve_batch`` solves many positions in one launch of the lane solver (csrc/rz_solver.cuh, up to 12
 empties); ``solve_deep_batch`` solves exact positions up to 30 empties one after another, each with the whole device
-(csrc/rz_solver_deep.cu)."""
+(csrc/rz_solver_deep.cu), which keeps a transposition table of proven bounds on the device across calls."""
+import ctypes as C
+
 import numpy as np
 
 from .. import _cabi
@@ -42,8 +44,27 @@ def solve_deep_batch(own, enemy, timeout=30.0, stats=False):
 
 
 def tune_deep(slice_us=0, leaf_target=0, leaf_floor=0):
-    """Slice length (us), split leaf target and leaf floor (empties) of the deep solver; 0 restores a default."""
+    """Slice length (us), split leaf target and leaf floor (empties) of the deep solver; 0 restores a default.  The next
+    solve starts from an empty transposition table."""
     _cabi.check(_cabi.lib().rz_solve_deep_tune(int(slice_us), int(leaf_target), int(leaf_floor)), "rz_solve_deep_tune")
+
+
+def deep_table_bytes(nbytes=0):
+    """Size of the deep solver's transposition table from its next call on (which starts empty); 0: the default 1 GiB."""
+    _cabi.check(_cabi.lib().rz_solve_deep_table(int(nbytes)), "rz_solve_deep_table")
+
+
+def clear_deep_table():
+    """Empty the deep solver's transposition table on the current device and zero its counts."""
+    _cabi.check(_cabi.lib().rz_solve_deep_clear(), "rz_solve_deep_clear")
+
+
+def deep_table_stats():
+    """Counts of the transposition table since the last clear: lookups, cutoffs, hints, stores, replaced, merges,
+    dropped, occupied (entries now) and bytes."""
+    st = _cabi.DeepTableStats()
+    _cabi.check(_cabi.lib().rz_solve_deep_table_stats(C.byref(st)), "rz_solve_deep_table_stats")
+    return {k: getattr(st, k) for k, _ in _cabi.DeepTableStats._fields_}
 
 
 class ReversiSolver:
