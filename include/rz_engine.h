@@ -102,6 +102,13 @@ typedef struct rz_deep_solve_stats {
 } rz_deep_solve_stats;
 int rz_solve_deep(const uint64_t* own, const uint64_t* enemy, int8_t* move, int8_t* score, size_t n, double timeout_s,
                   rz_deep_solve_stats* stats);
+/* rz_solve_deep with a stop flag owned by the caller (nullable; NULL is rz_solve_deep).  The flag is read before each
+ * position and wherever the timeout is checked, and may be set from another thread: once it is nonzero the call returns
+ * within one slice plus the host's split time, and every position not yet finished answers move -1, score 0, like a
+ * timeout.  The transposition table only ever holds proven bounds, so a stopped solve leaves nothing a later solve of
+ * the same position could be misled by. */
+int rz_solve_deep_with_stop(const uint64_t* own, const uint64_t* enemy, int8_t* move, int8_t* score, size_t n, double timeout_s,
+                            const volatile int32_t* stop, rz_deep_solve_stats* stats);
 /* Tuning of rz_solve_deep for tests and measurements: slice length (us), leaf target of the split and leaf floor
  * (empties below which the split stops); 0 restores each default (4000 us, one leaf per lane, 10 empties).  The next
  * call starts from an empty transposition table, so that it searches under the new tuning. */
@@ -368,6 +375,17 @@ int rz_engine_set_resign_threshold(rz_engine* e, int use_resign_threshold, float
  * persists across the moves of a game, agent/player.py:44-47); 0 starts from an empty table. */
 int rz_engine_search_root(rz_engine* e, uint64_t own, uint64_t enemy, int player, int slot, int keep_tree,
                           int32_t* n_visit, float* w_sum);
+/* one root per slot (whole-game analysis): slot i < n searches (own[i], enemy[i]) -- host arrays, mover's frame -- with
+ * player[i] (1 or 2) to move for simulation_num_per_move simulations; slots n .. games-1 stay idle and take no tower rows.
+ * keep_tree as in rz_engine_search_root, per slot, so repeated calls with keep_tree = 1 continue every slot's tree (a
+ * search in chunks).  Returns the root statistics of the n slots: n_visit[n][64], w_sum[n][64].  With noise_eps = 0 every
+ * slot uses the game id first_game_id, so slot i gives the same bits as a one-slot engine of the same configuration
+ * running rz_engine_search_root on that position, whatever the other slots hold; with root noise, slot i uses the game
+ * id first_game_id + i * game_id_stride (a one-slot engine created with that first_game_id reproduces it).
+ * RZ_EINVAL, with the engine left usable: n outside 1..games, a player other than 1 or 2, or a root without a legal
+ * move for its mover (passes and finished games are the caller's). */
+int rz_engine_search_roots(rz_engine* e, const uint64_t* own, const uint64_t* enemy, const uint8_t* player, int n,
+                           int keep_tree, int32_t* n_visit, float* w_sum);
 
 /* ------------------------------------------------------------------------------------------------
  * play_data writer -- the reference's output contract (worker/self_play.py:180-194,

@@ -200,13 +200,25 @@ __global__ void init_slots_kernel(const DevCfg c, const DevPtrs p) {
     p.mail_flag[(size_t)s * 2] = 0; p.mail_flag[(size_t)s * 2 + 1] = 0;
 }
 
-// test hook: every slot searches the same root once (no game loop); one warp per slot like the tick kernel
-__global__ void setup_search_root_kernel(const DevCfg c, const DevPtrs p, u64 own, u64 enemy, int pid, int keep_tree) {
+// single-position searches (rz_engine_search_root / rz_engine_search_roots): slot s < n_active searches roots[s], or roots[0]
+// when there is one root, once (no game loop); the other slots go idle at once.  One warp per slot like the tick kernel.
+// gid_stride: slot s draws the game id first_game_id + s * gid_stride (dihedral of each leaf evaluation, root noise).
+struct Root { u64 own, enemy; uint32_t pid, pad; };
+
+__global__ void setup_search_root_kernel(const DevCfg c, const DevPtrs p, const Root* __restrict__ roots, int n_roots, int n_active,
+                                         u64 gid_stride, int keep_tree) {
     const int s = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
     if (s >= c.G) return;
+    if (s >= n_active) {
+        if (lane == 0) { p.slots[s].phase = PH_IDLE; atomicAdd(&p.status->idle_slots, 1ULL); }
+        return;
+    }
+    const Root r = roots[n_roots > 1 ? s : 0];
+    const u64 own = r.own, enemy = r.enemy;
+    const int pid = (int)r.pid;
     WCtx x(c, p, s, lane);
     Slot& sl = x.sl;
-    sl.game_id = c.first_game_id + (u64)s * c.game_id_stride;
+    sl.game_id = c.first_game_id + (u64)s * gid_stride;
     if (!keep_tree || sl.gen == 0) {
         sl.gen = sl.gen + 1;
         if (sl.gen >= 4096) {
@@ -223,8 +235,10 @@ __global__ void setup_search_root_kernel(const DevCfg c, const DevPtrs p, u64 ow
     sl.search_only = 1;
     x.write_back();
 }
-__global__ void read_root_kernel(const DevCfg c, const DevPtrs p, int s, int32_t* n_out, float* w_out) {
-    WCtx x(c, p, s, (int)threadIdx.x);
+// root statistics of slots s0 .. s0 + gridDim.x - 1, one warp per slot, into rows 0 .. gridDim.x - 1 of n_out / w_out
+__global__ void read_root_kernel(const DevCfg c, const DevPtrs p, int s0, int32_t* n_out, float* w_out) {
+    WCtx x(c, p, s0 + (int)blockIdx.x, (int)threadIdx.x);
+    n_out += (size_t)blockIdx.x * 64; w_out += (size_t)blockIdx.x * 64;
     n_out[threadIdx.x] = 0; n_out[threadIdx.x + 32] = 0; w_out[threadIdx.x] = 0.f; w_out[threadIdx.x + 32] = 0.f;
     __syncwarp();
     const int ni = x.find_node(x.sl.root_own, x.sl.root_enemy, x.kpid_of(x.sl.root_pid));
@@ -273,6 +287,9 @@ struct rz_engine {
     int ev_used;
     double nn_ms, mcts_ms, run_ms;
     uint32_t cache_sets;  // sets of the evaluation cache (0: off); dp.cache.n_sets is 0 while two networks play
+    Root* d_roots;        // single-position searches: [G] roots, [G][64] root statistics (allocated on first use)
+    int32_t* d_root_n;
+    float* d_root_w;
 };
 
 constexpr int64_t kDefaultEvalCacheMb = 2048;
@@ -403,6 +420,36 @@ static int read_status(rz_engine* e) {
     return RZ_OK;
 }
 
+// Single-position searches: slots 0 .. n_active - 1 search their roots (see setup_search_root_kernel), then the root
+// statistics of slots read0 .. read0 + n_read - 1 come back in one readout launch and one copy per array.
+static int search_slots(rz_engine* e, const Root* roots, int n_roots, int n_active, u64 gid_stride, int keep_tree, int read0,
+                        int n_read, int32_t* n_visit, float* w_sum) {
+    const size_t G = (size_t)e->dc.G;
+    RZ_CUDA_TRY(cudaSetDevice(e->device));
+    RZ_TRY(sync_all(e));
+    if (!e->d_roots) {
+        RZ_TRY(dev_alloc(e, (void**)&e->d_roots, G * sizeof(Root), false));
+        RZ_TRY(dev_alloc(e, (void**)&e->d_root_n, G * 64 * sizeof(int32_t), false));
+        RZ_TRY(dev_alloc(e, (void**)&e->d_root_w, G * 64 * sizeof(float), false));
+    }
+    RZ_CUDA_TRY(cudaMemcpyAsync(e->d_roots, roots, (size_t)n_roots * sizeof(Root), cudaMemcpyHostToDevice, e->stream));
+    RZ_CUDA_TRY(cudaMemsetAsync(e->dp.status, 0, sizeof(Status), e->stream));
+    setup_search_root_kernel<<<(e->dc.G + 3) / 4, 128, 0, e->stream>>>(e->dc, e->dp, e->d_roots, n_roots, n_active, gid_stride, keep_tree);
+    RZ_LAUNCH_CHECK();
+    RZ_CUDA_TRY(cudaStreamSynchronize(e->stream));
+    for (int it = 0; it < 1000000; ++it) {
+        for (int i = 0; i < 8; ++i) RZ_TRY(launch_wave(e));
+        RZ_TRY(read_status(e));
+        if (e->h_status->idle_slots >= (unsigned long long)e->dc.G) break;
+    }
+    read_root_kernel<<<n_read, 32, 0, e->stream>>>(e->dc, e->dp, read0, e->d_root_n, e->d_root_w);
+    RZ_LAUNCH_CHECK();
+    RZ_CUDA_TRY(cudaMemcpyAsync(n_visit, e->d_root_n, (size_t)n_read * 64 * sizeof(int32_t), cudaMemcpyDeviceToHost, e->stream));
+    RZ_CUDA_TRY(cudaMemcpyAsync(w_sum, e->d_root_w, (size_t)n_read * 64 * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
+    RZ_CUDA_TRY(cudaStreamSynchronize(e->stream));
+    return RZ_OK;
+}
+
 extern "C" {
 
 int rz_engine_create(const rz_engine_cfg* cfg, rz_net* net, int device, rz_engine** out) {
@@ -421,6 +468,7 @@ int rz_engine_create(const rz_engine_cfg* cfg, rz_net* net, int device, rz_engin
     e->h_status = nullptr; e->h_flags = nullptr; e->stream = nullptr; e->stream2 = nullptr;
     e->ev_used = 0; e->nn_ms = e->mcts_ms = e->run_ms = 0.0;
     e->cache_sets = 0;
+    e->d_roots = nullptr; e->d_root_n = nullptr; e->d_root_w = nullptr;
     for (int i = 0; i < 48; ++i) e->ev[i] = nullptr;
     e->ev_run[0] = e->ev_run[1] = e->ev_run[2] = nullptr;
     // two slot groups on two streams: the MCTS tick of one group can run while the network launch of the other is in flight,
@@ -682,27 +730,24 @@ int rz_engine_set_resign_threshold(rz_engine* e, int use_resign_threshold, float
 int rz_engine_search_root(rz_engine* e, uint64_t own, uint64_t enemy, int player, int slot, int keep_tree, int32_t* n_visit,
                           float* w_sum) {
     RZ_REQUIRE(e && n_visit && w_sum && (player == 1 || player == 2) && slot >= 0 && slot < e->dc.G, "rz_engine_search_root: bad argument");
-    RZ_CUDA_TRY(cudaSetDevice(e->device));
-    RZ_TRY(sync_all(e));
-    RZ_CUDA_TRY(cudaMemsetAsync(e->dp.status, 0, sizeof(Status), e->stream));
-    setup_search_root_kernel<<<(e->dc.G + 3) / 4, 128, 0, e->stream>>>(e->dc, e->dp, own, enemy, player, keep_tree);
-    RZ_LAUNCH_CHECK();
-    RZ_CUDA_TRY(cudaStreamSynchronize(e->stream));
-    for (int it = 0; it < 1000000; ++it) {
-        for (int i = 0; i < 8; ++i) RZ_TRY(launch_wave(e));
-        RZ_TRY(read_status(e));
-        if (e->h_status->idle_slots >= (unsigned long long)e->dc.G) break;
+    const Root r{own, enemy, (uint32_t)player, 0};
+    return search_slots(e, &r, 1, e->dc.G, e->dc.game_id_stride, keep_tree, slot, 1, n_visit, w_sum);
+}
+
+int rz_engine_search_roots(rz_engine* e, const uint64_t* own, const uint64_t* enemy, const uint8_t* player, int n, int keep_tree,
+                           int32_t* n_visit, float* w_sum) {
+    RZ_REQUIRE(e && own && enemy && player && n_visit && w_sum, "rz_engine_search_roots: null pointer");
+    RZ_REQUIRE(n >= 1 && n <= e->dc.G, "rz_engine_search_roots: n = %d outside 1..%d (the engine's slots)", n, e->dc.G);
+    std::vector<Root> roots((size_t)n);
+    for (int i = 0; i < n; ++i) {
+        RZ_REQUIRE(player[i] == 1 || player[i] == 2, "rz_engine_search_roots: player[%d] = %d is not 1 or 2", i, (int)player[i]);
+        RZ_REQUIRE(find_correct_moves(own[i], enemy[i]) != 0, "rz_engine_search_roots: root %d has no legal move for its mover", i);
+        roots[(size_t)i] = Root{own[i], enemy[i], (uint32_t)player[i], 0};
     }
-    int32_t* d_n; float* d_w;
-    RZ_CUDA_TRY(cudaMalloc((void**)&d_n, 64 * 4));
-    RZ_CUDA_TRY(cudaMalloc((void**)&d_w, 64 * 4));
-    read_root_kernel<<<1, 32, 0, e->stream>>>(e->dc, e->dp, slot, d_n, d_w);
-    cudaError_t ce = cudaMemcpyAsync(n_visit, d_n, 256, cudaMemcpyDeviceToHost, e->stream);
-    if (ce == cudaSuccess) ce = cudaMemcpyAsync(w_sum, d_w, 256, cudaMemcpyDeviceToHost, e->stream);
-    if (ce == cudaSuccess) ce = cudaStreamSynchronize(e->stream);
-    cudaFree(d_n); cudaFree(d_w);
-    if (ce != cudaSuccess) { set_error("rz_engine_search_root: %s", cudaGetErrorString(ce)); return RZ_ECUDA; }
-    return RZ_OK;
+    // With root noise off the game id only picks the dihedral of each leaf evaluation: every slot then uses the first game
+    // id, so that a position gives the same statistics whatever slot it is searched in (those of a one-slot engine).
+    const u64 gid_stride = e->dc.noise_eps > 0.f ? e->dc.game_id_stride : 0;
+    return search_slots(e, roots.data(), n, n, gid_stride, keep_tree, 0, n, n_visit, w_sum);
 }
 
 }  // extern "C"

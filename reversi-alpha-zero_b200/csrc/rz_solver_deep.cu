@@ -278,7 +278,9 @@ struct Tree {
 struct ProbeRun {
     int slice_us, leaf_target, leaf_floor;
     std::chrono::steady_clock::time_point deadline;
+    const volatile int32_t* stop;  // the caller's stop flag (nullable): nonzero ends the call like a timeout
     rz_deep_solve_stats* stats;
+    bool expired() const { return (stop && *stop) || std::chrono::steady_clock::now() > deadline; }
 };
 
 static int upload_and_run(Workspace& w, Tree& T, const std::vector<int32_t>& claim, const std::vector<int32_t>& free_slots,
@@ -309,14 +311,15 @@ static int upload_and_run(Workspace& w, Tree& T, const std::vector<int32_t>& cla
     return RZ_OK;
 }
 
-// Decide the roots of T as far as the forest's question needs.  *timed_out is set when the deadline passed first.
+// Decide the roots of T as far as the forest's question needs.  *timed_out is set when the deadline passed, or the stop flag
+// was raised, first.
 static int run_forest(Workspace& w, Tree& T, const ProbeRun& P, bool* timed_out) {
     *timed_out = false;
     // split breadth-first, one level at a time, down to the leaf target or the leaf floor
     std::vector<int32_t> level, claim, free_slots;
     T.open_leaves(level);
     while (!T.answered() && T.leaves < P.leaf_target) {
-        if (std::chrono::steady_clock::now() > P.deadline) { *timed_out = true; return RZ_OK; }
+        if (P.expired()) { *timed_out = true; return RZ_OK; }
         bool grew = false;
         for (int c : level) {
             if (T.leaves >= P.leaf_target || T.nodes.size() + 64 > (size_t)kMaxNodes) break;
@@ -330,7 +333,7 @@ static int run_forest(Workspace& w, Tree& T, const ProbeRun& P, bool* timed_out)
     std::vector<int> order;
     std::vector<char> used(w.ctx_slots);
     while (!T.answered()) {
-        if (std::chrono::steady_clock::now() > P.deadline) { *timed_out = true; return RZ_OK; }
+        if (P.expired()) { *timed_out = true; return RZ_OK; }
         T.open_leaves(claim);
         if ((int)claim.size() < w.lanes) {  // lanes would sit idle: re-split the longest-running open leaves
             order.clear();
@@ -587,20 +590,22 @@ int rz_solve_deep_table_stats(rz_deep_table_stats* out) {
     return RZ_OK;
 }
 
-int rz_solve_deep(const uint64_t* own, const uint64_t* enemy, int8_t* move, int8_t* score, size_t n, double timeout_s,
-                  rz_deep_solve_stats* stats) {
+int rz_solve_deep_with_stop(const uint64_t* own, const uint64_t* enemy, int8_t* move, int8_t* score, size_t n, double timeout_s,
+                            const volatile int32_t* stop, rz_deep_solve_stats* stats) {
     RZ_REQUIRE(n == 0 || (own && enemy && move && score), "rz_solve_deep: null pointer");
     deep::Workspace* w = nullptr;
     if (n) RZ_TRY(deep::workspace(&w));
     for (size_t i = 0; i < n; ++i) {
+        if (stats) stats[i] = rz_deep_solve_stats{};
+        if (stop && *stop) { move[i] = -1; score[i] = 0; continue; }
         const auto t0 = std::chrono::steady_clock::now();
         deep::ProbeRun P;
         P.slice_us = deep::g_tuning.slice_us ? deep::g_tuning.slice_us : deep::kDefaultSliceUs;
         P.leaf_target = deep::g_tuning.leaf_target ? deep::g_tuning.leaf_target : w->lanes;
         P.leaf_floor = deep::g_tuning.leaf_floor ? deep::g_tuning.leaf_floor : deep::kDefaultLeafFloor;
         P.deadline = t0 + std::chrono::duration_cast<std::chrono::steady_clock::duration>(std::chrono::duration<double>(timeout_s));
+        P.stop = stop;
         P.stats = stats ? stats + i : nullptr;
-        if (P.stats) *P.stats = rz_deep_solve_stats{};
         unsigned long long steps0 = 0, steps1 = 0;
         if (P.stats) RZ_CUDA_TRY(cudaMemcpy(&steps0, w->total_steps, 8, cudaMemcpyDeviceToHost));
         RZ_TRY(deep::solve_one(*w, own[i], enemy[i], move + i, score + i, P));
@@ -611,6 +616,11 @@ int rz_solve_deep(const uint64_t* own, const uint64_t* enemy, int8_t* move, int8
         }
     }
     return RZ_OK;
+}
+
+int rz_solve_deep(const uint64_t* own, const uint64_t* enemy, int8_t* move, int8_t* score, size_t n, double timeout_s,
+                  rz_deep_solve_stats* stats) {
+    return rz_solve_deep_with_stop(own, enemy, move, score, n, timeout_s, nullptr, stats);
 }
 
 }  // extern "C"

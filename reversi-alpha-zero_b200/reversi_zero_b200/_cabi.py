@@ -91,6 +91,7 @@ SIGNATURES = {
     "rz_solve_dev": (C.c_int, [vp, vp, vp, vp, vp, sz, vp]),
     "rz_solve": (C.c_int, [u64p, u64p, u8p, i8p, i8p, sz]),
     "rz_solve_deep": (C.c_int, [u64p, u64p, i8p, i8p, sz, C.c_double, C.POINTER(DeepSolveStats)]),
+    "rz_solve_deep_with_stop": (C.c_int, [u64p, u64p, i8p, i8p, sz, C.c_double, C.POINTER(C.c_int32), C.POINTER(DeepSolveStats)]),
     "rz_solve_deep_tune": (C.c_int, [C.c_int, C.c_int, C.c_int]),
     "rz_solve_deep_table": (C.c_int, [C.c_int64]),
     "rz_solve_deep_clear": (C.c_int, []),
@@ -126,6 +127,7 @@ SIGNATURES = {
     "rz_engine_set_second_net": (C.c_int, [vp, vp, C.c_int]),
     "rz_engine_set_resign_threshold": (C.c_int, [vp, C.c_int, C.c_float]),
     "rz_engine_search_root": (C.c_int, [vp, C.c_uint64, C.c_uint64, C.c_int, C.c_int, C.c_int, i32p, f32p]),
+    "rz_engine_search_roots": (C.c_int, [vp, u64p, u64p, u8p, C.c_int, C.c_int, i32p, f32p]),
     "rz_write_play_data": (C.c_int, [C.c_char_p, C.POINTER(Game), sz, C.POINTER(Ply), C.c_int, C.c_int, C.POINTER(sz)]),
     "rz_write_play_rows": (C.c_int, [C.c_char_p, C.POINTER(Game), sz, C.POINTER(Ply), C.c_int, C.c_int, C.POINTER(sz)]),
     "rz_read_play_rows": (C.c_int, [C.c_char_p, vp, sz, C.POINTER(sz), C.POINTER(C.c_int), C.POINTER(C.c_int)]),

@@ -32,6 +32,19 @@ def solver_max_empties(config):
     return int(getattr(getattr(config, "b200", None), "solver_max_empties", 12))
 
 
+def search_play_config(config, play_config):
+    """The search parameters ReversiPlayer's engine runs with: `play_config`, except that the reference reads three of
+    them from config.play even when a separate play_config is given (evaluate.py / play_game callers):
+    allowed_resign_turn (agent/player.py:127, handled in action_with_evaluation), use_solver_turn_in_simulation
+    (:237-238) and virtual_loss (:264).  thinking_loop is at least 1 (the loop runs on the host, see there)."""
+    search_pc = SimpleNamespace(**vars(play_config))
+    for k in ("use_solver_turn_in_simulation", "virtual_loss"):
+        if hasattr(config.play, k):
+            setattr(search_pc, k, getattr(config.play, k))
+    search_pc.thinking_loop = max(1, int(search_pc.thinking_loop))
+    return search_pc
+
+
 class ReversiPlayer:
     def __init__(self, config, model, play_config=None, enable_resign=True, mtcs_info=None, api=None, seed=0, device=0):
         """model: a ``reversi_zero_b200.net.Net`` (None selects the deterministic test evaluator).
@@ -41,15 +54,7 @@ class ReversiPlayer:
         self.play_config = play_config or self.config.play
         self.enable_resign = enable_resign
         self.api = api
-        # The reference reads three search parameters from config.play even when a separate play_config is given
-        # (evaluate.py / play_game callers): allowed_resign_turn (agent/player.py:127, handled below),
-        # use_solver_turn_in_simulation (:237-238) and virtual_loss (:264).
-        search_pc = SimpleNamespace(**vars(self.play_config))
-        for k in ("use_solver_turn_in_simulation", "virtual_loss"):
-            if hasattr(self.config.play, k):
-                setattr(search_pc, k, getattr(self.config.play, k))
-        search_pc.thinking_loop = max(1, int(search_pc.thinking_loop))   # the loop runs on the host (below); see there
-        ecfg = engine_cfg_from_play_config(search_pc, games=1, seed=seed,
+        ecfg = engine_cfg_from_play_config(search_play_config(self.config, self.play_config), games=1, seed=seed,
                                            eval_mode=EVAL_NET if model is not None else EVAL_FAKE)
         self.engine = Engine(ecfg, model, device)
         self._fresh = True

@@ -133,6 +133,7 @@ class B200Config(_Section):
         self.train_from_json = False  # opt: parse play_*.json itself on the device and ignore the rows twins (worker/optimize.py)
         self.train_devices = None   # opt: CUDA ordinals of a data-parallel training group, e.g. [0, 1]; None = the one device
         self.solver_max_empties = 12  # ReversiPlayer's exact root solver: 13..this many empties go to the whole-GPU solver
+        self.nboard_analyze = False  # NBoard: answer `analyze` with a retrograde analysis of the game (play_game/analysis.py)
 
 
 class Config(_Section):

@@ -134,6 +134,22 @@ class Engine:
                                                        w.ctypes.data_as(_cabi.f32p)), "rz_engine_search_root")
         return n, w
 
+    def search_roots(self, own, enemy, player, keep_tree=False):
+        """One root per slot (rz_engine_search_roots): slot i searches (own[i], enemy[i]) in the mover's frame with
+        player[i] (1 or 2, or one value for all) to move.  -> (n int32 [len(own), 64], w float32 [len(own), 64])."""
+        own = np.ascontiguousarray(own, dtype=np.uint64).reshape(-1)
+        enemy = np.ascontiguousarray(enemy, dtype=np.uint64).reshape(-1)
+        pl = np.ascontiguousarray(np.broadcast_to(np.asarray(player, dtype=np.uint8), own.shape))
+        if enemy.shape != own.shape:
+            raise ValueError("own and enemy differ in length")
+        n = np.zeros((own.size, 64), np.int32)
+        w = np.zeros((own.size, 64), np.float32)
+        _cabi.check(_cabi.lib().rz_engine_search_roots(self._h, own.ctypes.data_as(_cabi.u64p), enemy.ctypes.data_as(_cabi.u64p),
+                                                        pl.ctypes.data_as(_cabi.u8p), int(own.size), int(keep_tree),
+                                                        n.ctypes.data_as(_cabi.i32p), w.ctypes.data_as(_cabi.f32p)),
+                    "rz_engine_search_roots")
+        return n, w
+
     def close(self):
         if self._h:
             _cabi.lib().rz_engine_destroy(self._h)

@@ -25,18 +25,25 @@ def solve_batch(own, enemy, exactly):
     return move, score
 
 
-def solve_deep_batch(own, enemy, timeout=30.0, stats=False):
+def solve_deep_batch(own, enemy, timeout=30.0, stats=False, stop=None):
     """Exact solve of each position (uint64 arrays in the mover's frame) with the whole device, one after another;
-    `timeout` seconds per position.  -> (move int8[], score int8[]) with move -1 = no legal move, more than 30 empties or
-    timed out; with stats=True also a list of dicts (probes, slices, resplits, leaves, node_steps, seconds)."""
+    `timeout` seconds per position.  -> (move int8[], score int8[]) with move -1 = no legal move, more than 30 empties,
+    timed out or stopped; with stats=True also a list of dicts (probes, slices, resplits, leaves, node_steps, seconds).
+    stop: a ``ctypes.c_int32`` another thread may set to nonzero to end the call within one slice
+    (rz_solve_deep_with_stop); the positions not finished by then answer like a timeout."""
     own = np.ascontiguousarray(own, dtype=np.uint64).reshape(-1)
     enemy = np.ascontiguousarray(enemy, dtype=np.uint64).reshape(-1)
     move = np.empty(own.shape, np.int8)
     score = np.empty(own.shape, np.int8)
     st = (_cabi.DeepSolveStats * max(1, own.size))()
-    _cabi.check(_cabi.lib().rz_solve_deep(own.ctypes.data_as(_cabi.u64p), enemy.ctypes.data_as(_cabi.u64p),
-                                           move.ctypes.data_as(_cabi.i8p), score.ctypes.data_as(_cabi.i8p), own.size,
-                                           float(timeout), st), "rz_solve_deep")
+    if stop is None:
+        _cabi.check(_cabi.lib().rz_solve_deep(own.ctypes.data_as(_cabi.u64p), enemy.ctypes.data_as(_cabi.u64p),
+                                               move.ctypes.data_as(_cabi.i8p), score.ctypes.data_as(_cabi.i8p), own.size,
+                                               float(timeout), st), "rz_solve_deep")
+    else:
+        _cabi.check(_cabi.lib().rz_solve_deep_with_stop(own.ctypes.data_as(_cabi.u64p), enemy.ctypes.data_as(_cabi.u64p),
+                                                         move.ctypes.data_as(_cabi.i8p), score.ctypes.data_as(_cabi.i8p), own.size,
+                                                         float(timeout), C.byref(stop), st), "rz_solve_deep_with_stop")
     if not stats:
         return move, score
     names = [f for f, _ in _cabi.DeepSolveStats._fields_ if f != "pad"]

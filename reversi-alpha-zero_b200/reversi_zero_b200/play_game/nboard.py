@@ -6,7 +6,8 @@ Commands arrive on stdin, one per line; stdout carries protocol replies only (lo
 ``run.py`` sets up).  ``go`` and ``hint`` search with the one-slot ``ReversiPlayer`` mirror, whose simulations run on
 the device; the tree is kept across the moves of a game and dropped when NBoard sends the opening position.  A
 ``ping`` interrupts a running search from the reader thread, so NBoard gets its ``pong`` as soon as the current chunk
-of ``hint_callback_per_sim`` simulations ends.
+of ``hint_callback_per_sim`` simulations ends.  With ``b200.nboard_analyze`` on, ``analyze`` answers with a retrograde
+analysis of the game (play_game/analysis.py), which a ``ping`` interrupts as well.
 """
 import re
 import sys
@@ -39,6 +40,10 @@ def start(config):
 
 
 class NBoardEngine:
+    # play_game.analysis.GameAnalyser, created at the first analysis.  A class attribute, so that the reader thread's
+    # push_callback finds it on every engine, also one whose analysis has never run.
+    analyser = None
+
     def __init__(self, config, stdin=None, stdout=None):
         self.config = config
         self.stdout = stdout or sys.stdout
@@ -51,6 +56,8 @@ class NBoardEngine:
         self.play_config = self.config.play
         self.player = self.create_player()
         self.turn_of_nboard = None
+        self.game_start = None      # (black, white, player) of `set game`, and the actions since: the game `analyze` analyses
+        self.game_actions = []
 
     def create_player(self):
         logger.debug("create new ReversiPlayer()")
@@ -76,6 +83,8 @@ class NBoardEngine:
         # called on the reader thread: a ping ends the running search
         if message.startswith("ping"):
             self.stop_thinking()
+            if self.analyser is not None:
+                self.analyser.stop()
 
     def stop(self):
         self.running = False
@@ -108,6 +117,8 @@ class NBoardEngine:
         self.env.reset()
         self.env.update(game_state.black, game_state.white, game_state.player)
         self.turn_of_nboard = game_state.player
+        self.game_start = (game_state.black, game_state.white, game_state.player)
+        self.game_actions = list(game_state.actions)
         for action in game_state.actions:
             self._change_turn()
             if action is not None:
@@ -118,6 +129,7 @@ class NBoardEngine:
             self.turn_of_nboard = Player.black if self.turn_of_nboard == Player.white else Player.white
 
     def move(self, action):
+        self.game_actions.append(action)
         self._change_turn()
         if action is not None:
             self.env.step(action)
@@ -148,6 +160,28 @@ class NBoardEngine:
         self.player.action(*states, callback_in_mtcs=CallbackInMCTS(self.nc.hint_callback_per_sim, hint_report_callback))
         item = self.player.ask_thought_about(*states)
         hint_report_callback(item.values, item.visit)
+
+
+    def begin_analysis(self):
+        """before `status analyzing...`: the analyser exists and no earlier ping stops the analysis about to start"""
+        if self.analyser is None:
+            from .analysis import GameAnalyser
+            self.analyser = GameAnalyser(self.config, self.model, self.play_config)
+        self.analyser.reset_stop()
+
+    def analyze(self, report):
+        """report(moves_made, value, exact) for every position of the game since `set game`, until a ping stops it"""
+        if self.game_start is None:
+            return
+        black, white, player = self.game_start
+        self.analyser.analyse(black, white, player, self.game_actions, report)
+
+
+def analysis_line(moves_made, value, exact):
+    """NBoard's `analysis {movesMade} {eval}` line.  `value` is from the viewpoint of the side to move in that position,
+    like the `===` and `search` lines (INTEGRATION §5); exact values (final disc differences) print as integers, searched
+    ones (10 * q) in `go`'s float format."""
+    return f"analysis {moves_made} {int(value) if exact else float(value)}"
 
 
 class NBoardProtocolVersion2:
@@ -224,8 +258,17 @@ class NBoardProtocolVersion2:
         self.engine.reply("learned")
 
     def analyze(self):
-        """Retrograde analysis is optional in the protocol; the reference leaves it out as well."""
-        pass
+        """Retrograde analysis is optional in the protocol and the reference leaves it out; with b200.nboard_analyze on,
+        one `analysis` line per position between `status analyzing...` and `status waiting`."""
+        if not getattr(getattr(self.config, "b200", None), "nboard_analyze", False):
+            return
+        self.engine.begin_analysis()
+        self.tell_status("analyzing...")
+        self.engine.analyze(self.report_analysis)
+        self.tell_status("waiting")
+
+    def report_analysis(self, moves_made, value, exact):
+        self.engine.reply(analysis_line(moves_made, value, exact))
 
     def tell_status(self, status):
         self.engine.reply(f"status {status}")
