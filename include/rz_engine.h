@@ -305,8 +305,9 @@ typedef struct rz_game {
     uint8_t resign_enabled;
     uint8_t resigned_mask;  /* bit0 black wanted to resign, bit1 white */
     uint8_t turn;           /* ReversiEnv.turn at the end */
-    uint8_t black_net;      /* evaluation matches: 0 = black was played by the first network, 1 = by the second */
-    uint8_t pad[2];
+    uint8_t black_net;      /* matches and leagues: index of the network that played black (0 in self-play) */
+    uint8_t white_net;      /* ... and white (0 in self-play, 1 - black_net in a two-network match) */
+    uint8_t pad;
     int32_t table_nodes;    /* positions in the slot's statistics table at the end of the game (half of the reference's
                                len(mtcs_info.var_p), which also holds every colour-swapped mirror key, worker/self_play.py:127) */
     int32_t pad2;
@@ -365,6 +366,18 @@ int rz_engine_set_simulation_num(rz_engine* e, int32_t sims);
  * network" is the deterministic evaluator with the value negated.  NULL switches back to one network.  Call before
  * the first rz_engine_run. */
 int rz_engine_set_second_net(rz_engine* e, rz_net* net_b, int enable);
+/* leagues: up to RZ_MAX_NETS networks in one engine.  The game with local index i (< n_games) is played by
+ * nets[black_net[i]] as black and nets[white_net[i]] as white; every search is evaluated by the mover's own network, each
+ * network by its own implementation (widths and depths may differ).  The table (2 bytes per game) is copied to the
+ * device.  RZ_EVAL_FAKE: nets may be NULL, and network k is the deterministic evaluator with its value multiplied by
+ * fake_scale[k] (NULL: all 1).  rz_engine_set_second_net is the two-network case with no table (colours alternate with
+ * the local index, scales 1 and -1).  The evaluation cache stays off while more than one network is set.  Row buffers
+ * grow to n_nets x games x parallel_search_num rows (RZ_ENOMEM if that fails).  RZ_EINVAL, with the engine unchanged:
+ * n_nets outside 2..RZ_MAX_NETS, an index >= n_nets, a NULL network under RZ_EVAL_NET, max_games 0 or greater than
+ * n_games (rz_engine_set_max_games then keeps to that bound), or a call after the first wave. */
+#define RZ_MAX_NETS 16
+int rz_engine_set_nets(rz_engine* e, rz_net* const* nets, const float* fake_scale, int n_nets, const uint8_t* black_net,
+                       const uint8_t* white_net, uint64_t n_games);
 /* update the resignation rule for decisions taken from now on (SelfPlayWorker's threshold auto-tuner,
  * worker/self_play.py:250-260). */
 int rz_engine_set_resign_threshold(rz_engine* e, int use_resign_threshold, float resign_threshold);

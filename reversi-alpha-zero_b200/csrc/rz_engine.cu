@@ -118,7 +118,7 @@ struct Slot {
     uint8_t resigned_mask, search_only, n_pending, n_parked;
     uint8_t pending[kMaxK], parked[kMaxK];
     u64 root_own, root_enemy;
-    uint8_t root_pid, black_net, cur_net;  // black_net / cur_net: evaluation matches (two networks)
+    uint8_t root_pid, black_net, white_net;  // black_net / white_net: networks of the two colours (matches, leagues)
     uint8_t root_req;         // 1: an exact root solve has to be put into this wave's solver batch
     uint32_t ply_waves;       // waves this slot has spent on the ply being decided (rz_ply::waves)
     uint32_t n_solves, n_searched_plies;
@@ -137,7 +137,7 @@ struct Status {
 
 struct DevCfg {
     int G, S, K, vl, change_tau_turn, thinking_loop, required_visit, start_rethinking_turn, allowed_resign_turn;
-    int use_resign, share, max_plies, warm_start, sims_cap, two_nets, solver_turn, solver_sim_turn, keep_games;
+    int use_resign, share, max_plies, warm_start, sims_cap, n_nets, solver_turn, solver_sim_turn, keep_games;
     float c_puct, noise_eps, alpha, resign_threshold, disable_resignation_rate;
     u64 seed, first_game_id, game_id_stride, max_games;
     uint32_t nodes_cap, edges_cap, hash_cap;  // per slot (hash_cap is a power of two)
@@ -163,11 +163,12 @@ struct DevPtrs {
     rz_game* mail_hdr;     // [G][2]
     uint8_t* mail_flag;    // [G][2]  1 = finished game waiting for the host
     Status* status;
-    uint32_t* batch_count; // leaves in the current batch
-    u64* batch_own;        // [G*K] transformed, side-to-move frame
+    uint32_t* batch_count; // leaves in the current batch: [group][net], 64 words apart
+    u64* batch_own;        // [net][G*K] transformed, side-to-move frame
     u64* batch_enemy;
-    float* policy;         // [G*K][64]
-    float* value;          // [G*K]
+    float* policy;         // [net][G*K][64]
+    float* value;          // [net][G*K]
+    const uint8_t* net_table;  // [game][2]: networks of black and white (rz_engine_set_nets); NULL: alternate with the game
     // endgame solver: one resumable request context per descent (+ one per slot for the exact root solve), the lists of
     // unfinished requests (per group, double-buffered by wave parity) and the network results a waiting slot has to keep
     solver::SolveCtx* sctx;  // [G][K + 1]
@@ -181,13 +182,13 @@ struct DevPtrs {
 
 #include "rz_engine_warp.cuh"
 
-// RZ_EVAL_FAKE: policy 1/64, value (#own - #enemy)/64 (oracle/nn.py FakeNetAPI)
+// RZ_EVAL_FAKE: policy 1/64, value scale * (#own - #enemy)/64 (oracle/nn.py FakeNetAPI)
 __global__ void fake_eval_kernel(const u64* __restrict__ own, const u64* __restrict__ enemy, const uint32_t* __restrict__ count,
-                                 float* __restrict__ policy, float* __restrict__ value, float sign) {
+                                 float* __restrict__ policy, float* __restrict__ value, float scale) {
     const uint32_t n = *count;
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n * 64; i += gridDim.x * blockDim.x) {
         policy[i] = 1.0f / 64.0f;
-        if ((i & 63) == 0) value[i >> 6] = sign * ((float)(popc64(own[i >> 6]) - popc64(enemy[i >> 6])) / 64.0f);
+        if ((i & 63) == 0) value[i >> 6] = scale * ((float)(popc64(own[i >> 6]) - popc64(enemy[i >> 6])) / 64.0f);
     }
 }
 
@@ -263,8 +264,12 @@ struct rz_engine {
     rz_engine_cfg cfg;
     DevCfg dc;
     DevPtrs dp;
-    rz_net* net;
-    rz_net* net_b;  // evaluation matches: the second network (NULL in self-play)
+    rz_net* net;                    // the network given at creation (self-play)
+    rz_net* nets[RZ_MAX_NETS];      // the evaluators: nets[0] = net in self-play; matches and leagues set the list
+    float fake_scale[RZ_MAX_NETS];  // RZ_EVAL_FAKE: value scale of each network
+    int row_nets;                   // networks the row buffers and batch counters have room for
+    uint8_t* d_net_table;           // rz_engine_set_nets: [game][2] on the device (NULL: none)
+    uint64_t net_table_games;
     int device;
     cudaStream_t stream;      // group 0 + all host<->device traffic
     cudaStream_t stream2;     // group 1 (tick of one group overlaps the network launch of the other)
@@ -320,6 +325,59 @@ static int dev_alloc(rz_engine* e, void** ptr, size_t bytes, bool zero) {
     return RZ_OK;
 }
 
+// puts `fresh` in the place of *ptr in the allocation table (appends when *ptr is NULL) and frees the old buffer
+static int arena_swap(rz_engine* e, void** ptr, void* fresh) {
+    int i = 0;
+    while (i < e->n_arena && (!*ptr || e->arena[i] != *ptr)) ++i;
+    if (i == e->n_arena) {
+        if (e->n_arena >= (int)(sizeof(e->arena) / sizeof(e->arena[0]))) { set_error("rz_engine: allocation table full"); return RZ_ESTATE; }
+        e->n_arena++;
+    }
+    e->arena[i] = fresh;
+    if (*ptr) RZ_CUDA_TRY(cudaFree(*ptr));
+    *ptr = fresh;
+    return RZ_OK;
+}
+
+// room for n_nets networks in the row buffers and batch counters (they only grow); on failure the old buffers stay
+static int grow_rows(rz_engine* e, int n_nets) {
+    if (n_nets <= e->row_nets) return RZ_OK;
+    const size_t B = (size_t)n_nets * e->dc.G * e->dc.K;
+    DevPtrs& p = e->dp;
+    void** bufs[5] = {(void**)&p.batch_own, (void**)&p.batch_enemy, (void**)&p.policy, (void**)&p.value, (void**)&p.batch_count};
+    const size_t bytes[5] = {(B + 2) * sizeof(u64), (B + 2) * sizeof(u64), (B + 2) * 64 * sizeof(float), (B + 2) * sizeof(float),
+                             (size_t)n_nets * 2 * 64 * sizeof(uint32_t)};
+    void* fresh[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
+    for (int i = 0; i < 5; ++i) {
+        const cudaError_t ce = cudaMalloc(&fresh[i], bytes[i]);
+        if (ce != cudaSuccess) {
+            cudaGetLastError();
+            for (int j = 0; j < i; ++j) cudaFree(fresh[j]);
+            set_error("rz_engine: cudaMalloc(%zu bytes) for the rows of %d networks failed: %s", bytes[i], n_nets, cudaGetErrorString(ce));
+            return RZ_ENOMEM;
+        }
+    }
+    RZ_CUDA_TRY(cudaStreamSynchronize(e->stream));
+    for (int i = 0; i < 5; ++i) {
+        RZ_CUDA_TRY(cudaMemsetAsync(fresh[i], 0, bytes[i], e->stream));
+        RZ_TRY(arena_swap(e, bufs[i], fresh[i]));
+    }
+    e->row_nets = n_nets;
+    return RZ_OK;
+}
+
+// the evaluators from the next wave on: n networks (1: self-play with the creation network), an optional game table
+static void use_nets(rz_engine* e, rz_net* const* nets, const float* fake_scale, int n, const uint8_t* table) {
+    for (int k = 0; k < RZ_MAX_NETS; ++k) {
+        e->nets[k] = k < n && nets ? nets[k] : nullptr;
+        e->fake_scale[k] = k < n && fake_scale ? fake_scale[k] : 1.f;
+    }
+    if (n == 1) e->nets[0] = e->net;
+    e->dc.n_nets = n;
+    e->dp.net_table = table;
+    e->dp.cache.n_sets = n > 1 ? 0u : e->cache_sets;  // a leaf's result then depends on which network is to move
+}
+
 static int drain_mailboxes(rz_engine* e) {
     const int G = e->dc.G;
     RZ_CUDA_TRY(cudaMemcpyAsync(e->h_flags, e->dp.mail_flag, (size_t)G * 2, cudaMemcpyDeviceToHost, e->stream));
@@ -355,7 +413,7 @@ static int launch_wave(rz_engine* e) {
         cudaEvent_t* ev = e->ev + (g * 8 + e->ev_used) * 3;
         const size_t rows = (size_t)(s1 - s0) * c.K;
         if (timed) RZ_CUDA_TRY(cudaEventRecord(ev[0], st));
-        for (int net = 0; net <= c.two_nets; ++net) RZ_CUDA_TRY(cudaMemsetAsync(e->dp.batch_count + (net * 2 + g) * 64, 0, sizeof(uint32_t), st));
+        RZ_CUDA_TRY(cudaMemsetAsync(e->dp.batch_count + g * c.n_nets * 64, 0, ((c.n_nets - 1) * 64 + 1) * sizeof(uint32_t), st));
         const bool solving = c.solver_turn > 0 || c.solver_sim_turn > 0;
         const int par = e->solve_parity[g];  // the unfinished-solve list this wave's tick appends to
         if (solving) RZ_CUDA_TRY(cudaMemsetAsync(e->dp.solve_count + (g * 2 + (1 - par)) * 64, 0, sizeof(uint32_t), st));
@@ -373,16 +431,16 @@ static int launch_wave(rz_engine* e) {
             e->solve_parity[g] = 1 - par;
         }
         if (timed) RZ_CUDA_TRY(cudaEventRecord(ev[1], st));
-        for (int net = 0; net <= c.two_nets; ++net) {
-            uint32_t* count = e->dp.batch_count + (net * 2 + g) * 64;
+        for (int net = 0; net < c.n_nets; ++net) {  // one evaluator launch per network, on that network's rows
+            uint32_t* count = e->dp.batch_count + (g * c.n_nets + net) * 64;
             const size_t row0 = (size_t)net * c.G * c.K + (size_t)s0 * c.K;
             if (e->cfg.eval_mode == RZ_EVAL_FAKE) {
                 fake_eval_kernel<<<num_sms() * 4, 256, 0, st>>>(e->dp.batch_own + row0, e->dp.batch_enemy + row0, count, e->dp.policy + row0 * 64,
-                                                              e->dp.value + row0, net ? -1.f : 1.f);
+                                                              e->dp.value + row0, e->fake_scale[net]);
                 RZ_LAUNCH_CHECK();
                 e->mcts_launches++;
             } else {
-                RZ_TRY(net_forward_counted(net ? e->net_b : e->net, e->dp.batch_own + row0, e->dp.batch_enemy + row0, e->dp.policy + row0 * 64,
+                RZ_TRY(net_forward_counted(e->nets[net], e->dp.batch_own + row0, e->dp.batch_enemy + row0, e->dp.policy + row0 * 64,
                                            e->dp.value + row0, count, rows, e->cfg.net_impl, st));
                 e->nn_launches++;
             }
@@ -391,7 +449,7 @@ static int launch_wave(rz_engine* e) {
         if (e->dp.cache.n_sets) {  // this wave's tower rows into the evaluation cache (outside the timed evaluation)
             cache_insert_kernel<<<num_sms() * 2, 256, 0, st>>>(e->dp.cache, e->dp.batch_own + (size_t)s0 * c.K, e->dp.batch_enemy + (size_t)s0 * c.K,
                                                               e->dp.policy + (size_t)s0 * c.K * 64, e->dp.value + (size_t)s0 * c.K,
-                                                              e->dp.batch_count + g * 64, &e->dp.status->cache_repeats);
+                                                              e->dp.batch_count + g * c.n_nets * 64, &e->dp.status->cache_repeats);
             RZ_LAUNCH_CHECK();
             e->mcts_launches++;
         }
@@ -463,7 +521,11 @@ int rz_engine_create(const rz_engine_cfg* cfg, rz_net* net, int device, rz_engin
     RZ_CUDA_TRY(cudaSetDevice(device));
     rz_engine* e = new (std::nothrow) rz_engine();
     if (!e) { set_error("out of host memory"); return RZ_ENOMEM; }
-    e->cfg = *cfg; e->net = net; e->net_b = nullptr; e->device = device; e->n_arena = 0;
+    e->cfg = *cfg; e->net = net; e->device = device; e->n_arena = 0;
+    for (int k = 0; k < RZ_MAX_NETS; ++k) { e->nets[k] = nullptr; e->fake_scale[k] = 1.f; }
+    e->nets[0] = net;
+    e->row_nets = 2;
+    e->d_net_table = nullptr; e->net_table_games = 0;
     e->waves = e->nn_launches = e->mcts_launches = e->finished_total = 0;
     e->h_status = nullptr; e->h_flags = nullptr; e->stream = nullptr; e->stream2 = nullptr;
     e->ev_used = 0; e->nn_ms = e->mcts_ms = e->run_ms = 0.0;
@@ -485,7 +547,7 @@ int rz_engine_create(const rz_engine_cfg* cfg, rz_net* net, int device, rz_engin
     c.use_resign = cfg->use_resign_threshold; c.share = cfg->share_mtcs_info; c.max_plies = cfg->max_plies > 0 ? cfg->max_plies : 64;
     c.warm_start = cfg->warm_start;
     for (int t = 0; t < 60; ++t) { c.warm_cdf[t] = t < 58 ? (float)(t + 1) / 58.f : 1.f; c.warm_waves[t] = 0.f; }  // default: turns 0..57 equally likely
-    c.two_nets = 0;
+    c.n_nets = 1;
     c.keep_games = cfg->reset_mtcs_info_per_game > 1 ? cfg->reset_mtcs_info_per_game : 1;
     c.solver_turn = cfg->use_solver_turn; c.solver_sim_turn = cfg->use_solver_turn_in_simulation;
     c.sims_cap = cfg->max_sims_per_wave > 0 ? cfg->max_sims_per_wave : 2 * cfg->parallel_search_num;
@@ -507,7 +569,7 @@ int rz_engine_create(const rz_engine_cfg* cfg, rz_net* net, int device, rz_engin
     cudaError_t ce = cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking);
     if (ce == cudaSuccess) ce = cudaStreamCreateWithFlags(&e->stream2, cudaStreamNonBlocking);
     if (ce != cudaSuccess) { set_error("cudaStreamCreate: %s", cudaGetErrorString(ce)); delete e; return RZ_ECUDA; }
-    const size_t G = c.G, B = 2 * G * c.K;  // rows for two networks (evaluation matches); self-play uses the first half
+    const size_t G = c.G, B = (size_t)e->row_nets * G * c.K;  // rows for two networks (evaluation matches); self-play uses the first part
     DevPtrs& p = e->dp;
     rc = dev_alloc(e, (void**)&p.slots, G * sizeof(Slot), true);
     if (!rc) rc = dev_alloc(e, (void**)&p.desc, G * c.K * sizeof(Descent), true);
@@ -518,7 +580,8 @@ int rz_engine_create(const rz_engine_cfg* cfg, rz_net* net, int device, rz_engin
     if (!rc) rc = dev_alloc(e, (void**)&p.mail_hdr, G * 2 * sizeof(rz_game), true);
     if (!rc) rc = dev_alloc(e, (void**)&p.mail_flag, G * 2, true);
     if (!rc) rc = dev_alloc(e, (void**)&p.status, sizeof(Status), true);
-    if (!rc) rc = dev_alloc(e, (void**)&p.batch_count, 1024, true);
+    p.net_table = nullptr;
+    if (!rc) rc = dev_alloc(e, (void**)&p.batch_count, (size_t)e->row_nets * 2 * 64 * sizeof(uint32_t), true);
     if (!rc) rc = dev_alloc(e, (void**)&p.batch_own, (B + 2) * sizeof(u64), true);
     if (!rc) rc = dev_alloc(e, (void**)&p.batch_enemy, (B + 2) * sizeof(u64), true);
     if (!rc) rc = dev_alloc(e, (void**)&p.policy, (B + 2) * 64 * sizeof(float), true);
@@ -685,6 +748,9 @@ int rz_engine_set_simulation_num(rz_engine* e, int32_t sims) {
 
 int rz_engine_set_max_games(rz_engine* e, uint64_t max_games) {
     RZ_REQUIRE(e, "rz_engine_set_max_games: null engine");
+    RZ_REQUIRE(!e->dp.net_table || (max_games >= 1 && max_games <= e->net_table_games),
+               "rz_engine_set_max_games: %llu games with a network table of %llu games", (unsigned long long)max_games,
+               (unsigned long long)e->net_table_games);
     e->dc.max_games = max_games;
     e->cfg.max_games = max_games;
     return RZ_OK;
@@ -712,9 +778,45 @@ int rz_engine_set_second_net(rz_engine* e, rz_net* net_b, int enable) {
     RZ_REQUIRE(e, "rz_engine_set_second_net: null engine");
     RZ_REQUIRE(!enable || e->cfg.eval_mode == RZ_EVAL_FAKE || net_b, "rz_engine_set_second_net: a second network is required");
     RZ_REQUIRE(e->waves == 0, "rz_engine_set_second_net: must be called before the first wave");
-    e->net_b = enable ? net_b : nullptr;
-    e->dc.two_nets = enable ? 1 : 0;
-    e->dp.cache.n_sets = enable ? 0u : e->cache_sets;  // a leaf's result then depends on which network is to move
+    rz_net* const nets[2] = {e->net, net_b};
+    const float scale[2] = {1.f, -1.f};
+    use_nets(e, nets, scale, enable ? 2 : 1, nullptr);
+    return RZ_OK;
+}
+
+int rz_engine_set_nets(rz_engine* e, rz_net* const* nets, const float* fake_scale, int n_nets, const uint8_t* black_net,
+                       const uint8_t* white_net, uint64_t n_games) {
+    RZ_REQUIRE(e && black_net && white_net, "rz_engine_set_nets: null pointer");
+    RZ_REQUIRE(e->waves == 0, "rz_engine_set_nets: must be called before the first wave");
+    RZ_REQUIRE(n_nets >= 2 && n_nets <= RZ_MAX_NETS, "rz_engine_set_nets: n_nets = %d outside 2..%d", n_nets, RZ_MAX_NETS);
+    if (e->cfg.eval_mode == RZ_EVAL_NET) {
+        RZ_REQUIRE(nets, "rz_engine_set_nets: networks are required unless eval_mode == RZ_EVAL_FAKE");
+        for (int k = 0; k < n_nets; ++k) RZ_REQUIRE(nets[k], "rz_engine_set_nets: network %d is NULL", k);
+    }
+    RZ_REQUIRE(e->dc.max_games >= 1 && e->dc.max_games <= n_games,
+               "rz_engine_set_nets: max_games = %llu must be 1..n_games (%llu): the table has no entry for later games",
+               (unsigned long long)e->dc.max_games, (unsigned long long)n_games);
+    std::vector<uint8_t> table((size_t)n_games * 2);
+    for (uint64_t i = 0; i < n_games; ++i) {
+        RZ_REQUIRE(black_net[i] < n_nets && white_net[i] < n_nets, "rz_engine_set_nets: game %llu: networks %d / %d, but n_nets = %d",
+                   (unsigned long long)i, (int)black_net[i], (int)white_net[i], n_nets);
+        table[2 * i] = black_net[i];
+        table[2 * i + 1] = white_net[i];
+    }
+    RZ_CUDA_TRY(cudaSetDevice(e->device));
+    uint8_t* d_table = nullptr;
+    if (cudaMalloc((void**)&d_table, table.size()) != cudaSuccess) {
+        cudaGetLastError();
+        set_error("rz_engine_set_nets: cudaMalloc(%zu bytes) failed", table.size());
+        return RZ_ENOMEM;
+    }
+    int rc = grow_rows(e, n_nets);
+    if (rc) { cudaFree(d_table); return rc; }
+    RZ_CUDA_TRY(cudaMemcpyAsync(d_table, table.data(), table.size(), cudaMemcpyHostToDevice, e->stream));
+    RZ_CUDA_TRY(cudaStreamSynchronize(e->stream));
+    RZ_TRY(arena_swap(e, (void**)&e->d_net_table, d_table));
+    e->net_table_games = n_games;
+    use_nets(e, nets, fake_scale, n_nets, e->d_net_table);
     return RZ_OK;
 }
 

@@ -368,7 +368,6 @@ struct WCtx {
 
     __device__ void begin_search(u64 own, u64 enemy, int pid) {
         sl.root_own = own; sl.root_enemy = enemy; sl.root_pid = (uint8_t)pid;
-        sl.cur_net = c.two_nets ? (uint8_t)(pid == 1 ? sl.black_net : 1 - sl.black_net) : (uint8_t)0;
         sl.sims_started = 0; sl.sims_target = (uint32_t)c.S;
         sl.n_pending = 0; sl.n_parked = 0;
         sl.phase = PH_SEARCH;
@@ -438,7 +437,13 @@ struct WCtx {
             return;
         }
         sl.game_id = c.first_game_id + local * c.game_id_stride;
-        sl.black_net = c.two_nets ? (uint8_t)(local & 1) : (uint8_t)0;
+        if (p.net_table) {  // rz_engine_set_nets (max_games bounds `local` by the table's length)
+            sl.black_net = p.net_table[2 * local];
+            sl.white_net = p.net_table[2 * local + 1];
+        } else {  // self-play: network 0; two networks without a table: colours alternate with the game
+            sl.black_net = c.n_nets > 1 ? (uint8_t)(local & 1) : (uint8_t)0;
+            sl.white_net = c.n_nets > 1 ? (uint8_t)(1 - sl.black_net) : (uint8_t)0;
+        }
         sl.games_played++;
         env_reset(sl.env);
         if (c.keep_games > 1 && (sl.games_played - 1) % (u64)c.keep_games != 0) {
@@ -509,7 +514,7 @@ struct WCtx {
             g.first_ply = 0; g.n_plies = (int32_t)sl.ply; g.expansions = (int32_t)sl.n_expand; g.simulations = (int32_t)sl.n_sims;
             g.winner = sl.env.winner; g.black_z = sl.env.winner == 1 ? 1 : (sl.env.winner == 2 ? -1 : 0);
             g.resign_enabled = sl.enable_resign; g.resigned_mask = sl.resigned_mask; g.turn = sl.env.turn;
-            g.black_net = sl.black_net; g.pad[0] = g.pad[1] = 0;
+            g.black_net = sl.black_net; g.white_net = sl.white_net; g.pad = 0;
             g.table_nodes = (int32_t)sl.n_nodes; g.pad2 = 0;
             atomicMax(&p.status->max_nodes, (unsigned long long)sl.n_nodes);
             atomicMax(&p.status->max_edges, (unsigned long long)sl.n_edges);
@@ -708,11 +713,11 @@ __global__ void __launch_bounds__(kWarpTickThreads) tick_warp_kernel(const DevCf
         }
         if (n_nn) atomicAdd(&p.status->tower_rows, (unsigned long long)n_nn);
     }
-    const uint32_t net = c.two_nets ? sl.cur_net : 0u;  // evaluation matches: every search is evaluated by the mover's network
+    const uint32_t net = sl.root_pid == 1 ? sl.black_net : sl.white_net;  // the searching player's network (0 in self-play)
     uint32_t base = 0, sbase = 0;
     uint32_t* s_count = p.solve_count + (group * 2 + parity) * 64;
     uint32_t* s_list = p.sactive + (size_t)(group * 2 + parity) * c.G * (c.K + 1);
-    if (lane == 0 && n_nn > 0) base = atomicAdd(p.batch_count + (net * 2 + group) * 64, n_nn);
+    if (lane == 0 && n_nn > 0) base = atomicAdd(p.batch_count + (group * c.n_nets + net) * 64, n_nn);
     if (lane == 0 && n_sv > 0) sbase = atomicAdd(s_count, n_sv);
     base = __shfl_sync(0xffffffffu, base, 0);
     sbase = __shfl_sync(0xffffffffu, sbase, 0);

@@ -51,7 +51,7 @@ class Game(C.Structure):
     _fields_ = [("game_id", C.c_uint64), ("black", C.c_uint64), ("white", C.c_uint64), ("first_ply", C.c_int32),
                 ("n_plies", C.c_int32), ("expansions", C.c_int32), ("simulations", C.c_int32), ("winner", C.c_uint8),
                 ("black_z", C.c_int8), ("resign_enabled", C.c_uint8), ("resigned_mask", C.c_uint8), ("turn", C.c_uint8),
-                ("black_net", C.c_uint8), ("pad", C.c_uint8 * 2), ("table_nodes", C.c_int32), ("pad2", C.c_int32)]
+                ("black_net", C.c_uint8), ("white_net", C.c_uint8), ("pad", C.c_uint8), ("table_nodes", C.c_int32), ("pad2", C.c_int32)]
 
 
 class PlayRow(C.Structure):
@@ -125,6 +125,7 @@ SIGNATURES = {
     "rz_engine_set_warm_start_profile": (C.c_int, [vp, f32p, C.c_int]),
     "rz_engine_set_max_games": (C.c_int, [vp, C.c_uint64]),
     "rz_engine_set_second_net": (C.c_int, [vp, vp, C.c_int]),
+    "rz_engine_set_nets": (C.c_int, [vp, C.POINTER(vp), f32p, C.c_int, u8p, u8p, C.c_uint64]),
     "rz_engine_set_resign_threshold": (C.c_int, [vp, C.c_int, C.c_float]),
     "rz_engine_search_root": (C.c_int, [vp, C.c_uint64, C.c_uint64, C.c_int, C.c_int, C.c_int, i32p, f32p]),
     "rz_engine_search_roots": (C.c_int, [vp, u64p, u64p, u8p, C.c_int, C.c_int, i32p, f32p]),

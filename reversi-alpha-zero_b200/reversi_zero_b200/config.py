@@ -134,6 +134,18 @@ class B200Config(_Section):
         self.train_devices = None   # opt: CUDA ordinals of a data-parallel training group, e.g. [0, 1]; None = the one device
         self.solver_max_empties = 12  # ReversiPlayer's exact root solver: 13..this many empties go to the whole-GPU solver
         self.nboard_analyze = False  # NBoard: answer `analyze` with a retrograde analysis of the game (play_game/analysis.py)
+        self.keep_promoted_models = False  # eval: archive every promoted blob under <model_dir>/promoted/ (worker/evaluate.py)
+
+
+class LeagueConfig(_Section):
+    """Round-robin between saved models with Elo ratings (`league` command, worker/league.py)"""
+
+    def __init__(self):
+        self.models = None          # blob paths / globs relative to the project directory, or {path:, model: {...}} mappings;
+                                    # None = <model_dir>/promoted/*.rzblob.npy
+        self.game_num_per_pair = 100
+        self.play_config = None     # overrides of the evaluation play configuration
+        self.anchor = 0             # index of the model whose rating is fixed at 0
 
 
 class Config(_Section):
@@ -147,6 +159,7 @@ class Config(_Section):
         self.play_with_human = PlayWithHumanConfig()
         self.nboard = NBoardConfig()
         self.b200 = B200Config()
+        self.league = LeagueConfig()
 
 
 def create_config(d=None, project_dir=None, data_dir=None):

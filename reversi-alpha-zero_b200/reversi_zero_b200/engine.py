@@ -88,7 +88,7 @@ class Engine:
                 out.append(dict(game_id=int(g.game_id), black=int(g.black), white=int(g.white), winner=int(g.winner),
                                 black_z=int(g.black_z), expansions=int(g.expansions), simulations=int(g.simulations),
                                 resign_enabled=bool(g.resign_enabled), resigned_mask=int(g.resigned_mask), turn=int(g.turn),
-                                black_net=int(g.black_net), table_nodes=int(g.table_nodes), plies=pl))
+                                black_net=int(g.black_net), white_net=int(g.white_net), table_nodes=int(g.table_nodes), plies=pl))
         return out
 
     def stats(self):
@@ -121,6 +121,25 @@ class Engine:
         self.net_b = net_b  # keep alive
         _cabi.check(_cabi.lib().rz_engine_set_second_net(self._h, net_b.handle if net_b is not None else None, int(bool(enable))),
                     "rz_engine_set_second_net")
+
+    def set_nets(self, nets, black, white, fake_scales=None):
+        """leagues (rz_engine_set_nets): the game with local index i is played by nets[black[i]] as black and
+        nets[white[i]] as white.  ``nets`` may hold None with the deterministic evaluator, whose network k then has its
+        value multiplied by fake_scales[k] (None: all 1).  Call before the first run, with max_games in 1..len(black)."""
+        black = np.ascontiguousarray(black, dtype=np.uint8).reshape(-1)
+        white = np.ascontiguousarray(white, dtype=np.uint8).reshape(-1)
+        if black.shape != white.shape:
+            raise ValueError("black and white differ in length")
+        handles = (C.c_void_p * max(len(nets), 1))(*[n.handle if n is not None else None for n in nets])
+        scales = None
+        if fake_scales is not None:
+            sc = np.ascontiguousarray(fake_scales, dtype=np.float32)
+            if sc.size != len(nets):
+                raise ValueError("one fake scale per network")
+            scales = sc.ctypes.data_as(_cabi.f32p)
+        _cabi.check(_cabi.lib().rz_engine_set_nets(self._h, handles, scales, len(nets), black.ctypes.data_as(_cabi.u8p),
+                                                    white.ctypes.data_as(_cabi.u8p), int(black.size)), "rz_engine_set_nets")
+        self.nets = list(nets)  # keep alive
 
     def set_resign_threshold(self, threshold):
         _cabi.check(_cabi.lib().rz_engine_set_resign_threshold(self._h, 0 if threshold is None else 1,

@@ -1,8 +1,9 @@
 """Command line of the reference (run.py + manager.py):
 
-    python -m reversi_zero_b200.run {self,opt,eval,nboard} [-c config.yml] [--new] [--total-step N]
+    python -m reversi_zero_b200.run {self,opt,eval,nboard,league} [-c config.yml] [--new] [--total-step N]
 
-``self`` plays games, ``opt`` trains, ``eval`` promotes, ``nboard`` speaks the NBoard protocol on stdin / stdout.
+``self`` plays games, ``opt`` trains, ``eval`` promotes, ``nboard`` speaks the NBoard protocol on stdin / stdout,
+``league`` rates saved models against each other (settings in the YAML ``league:`` section).
 Files go under the project directory: ``$PROJECT_DIR``, else the current directory.  Every command logs to
 ``logs/main.log``; all but ``nboard`` also log to stderr.
 """
@@ -13,7 +14,7 @@ from .config import create_config, load_yaml
 
 logger = getLogger(__name__)
 
-CMD_LIST = ['self', 'opt', 'eval', 'nboard']
+CMD_LIST = ['self', 'opt', 'eval', 'nboard', 'league']
 
 
 def create_parser():
@@ -77,6 +78,9 @@ def start(argv=None):
     elif args.cmd == 'nboard':
         from .play_game import nboard
         return nboard.start(config)
+    elif args.cmd == 'league':
+        from .worker import league
+        return league.start(config)
 
 
 if __name__ == "__main__":

@@ -8,8 +8,10 @@ network, colours alternate by game index (the reference draws them at random, :7
 statistics (``share_mtcs_info = 0``, as ``ReversiPlayer(config, model, play_config=...)`` does in :69-70).  The
 verdict follows the reference's sequential bookkeeping (:44-64) over the games in game-index order, including its
 early-stop rules -- games after the point where the reference would have stopped do not count.  Weights are exchanged as float32 blobs (``*.rzblob.npy``, DESIGN.md section 9)."""
+import hashlib
 import os
 import shutil
+from datetime import datetime
 from glob import glob
 from logging import getLogger
 from time import sleep
@@ -24,6 +26,7 @@ from .self_play import blob_path_of
 logger = getLogger(__name__)
 
 NEXT_GENERATION_BLOB = "model_weight.rzblob.npy"
+PROMOTED_DIR = "promoted"  # under the model directory: every promoted blob, when b200.keep_promoted_models is on
 
 
 def start(config):
@@ -117,6 +120,8 @@ class EvaluateWorker:
 
     def start(self, max_models=None):
         self.best_net = self._load(blob_path_of(self.config))
+        if self._keep_promoted():
+            self.archive_best_model()
         done = 0
         while max_models is None or done < max_models:
             model_dir = self.next_generation_dir()
@@ -136,12 +141,42 @@ class EvaluateWorker:
         (worker/optimize.py load_model) and load_best_model_weight read -- when the trainer put them into the directory."""
         rc = self.config.resource
         shutil.copyfile(os.path.join(model_dir, NEXT_GENERATION_BLOB), blob_path_of(self.config))
+        if self._keep_promoted():
+            self._archive(os.path.join(model_dir, NEXT_GENERATION_BLOB), os.path.basename(os.path.normpath(model_dir)))
         for name, dst in ((rc.next_generation_model_config_filename, rc.model_best_config_path),
                           (rc.next_generation_model_weight_filename, rc.model_best_weight_path)):
             src = os.path.join(model_dir, name)
             if os.path.exists(src):
                 shutil.copyfile(src, dst + ".tmp")
                 os.replace(dst + ".tmp", dst)
+
+    def _keep_promoted(self):
+        return bool(getattr(getattr(self.config, "b200", None), "keep_promoted_models", False))
+
+    def _archive(self, src, name):
+        """copies the blob `src` to <model_dir>/promoted/<name>.rzblob.npy (a temporary file, then an atomic rename), so
+        that a league (worker/league.py) can rate every generation"""
+        d = os.path.join(self.config.resource.model_dir, PROMOTED_DIR)
+        os.makedirs(d, exist_ok=True)
+        dst = os.path.join(d, name + ".rzblob.npy")
+        shutil.copyfile(src, dst + ".tmp")
+        os.replace(dst + ".tmp", dst)
+        return dst
+
+    def archive_best_model(self):
+        """archives the current best blob as promoted/model_<its mtime>.rzblob.npy, unless a promoted blob with the same
+        content is there already: the first generation is then rated too"""
+        src = blob_path_of(self.config)
+
+        def digest(path):
+            with open(path, "rb") as f:
+                return hashlib.sha256(f.read()).hexdigest()
+        mine = digest(src)
+        for p in sorted(glob(os.path.join(self.config.resource.model_dir, PROMOTED_DIR, "*.rzblob.npy"))):
+            if digest(p) == mine:
+                return None
+        stamp = datetime.fromtimestamp(os.path.getmtime(src)).strftime("%Y%m%d-%H%M%S.%f")
+        return self._archive(src, self.config.resource.next_generation_model_dirname_tmpl % stamp)
 
     def remove_model(self, model_dir):
         """worker/evaluate.py:115-121: the reference removes its two files and then the directory (os.rmdir fails, loudly,
