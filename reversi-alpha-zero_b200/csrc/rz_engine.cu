@@ -440,8 +440,8 @@ static int launch_wave(rz_engine* e) {
                 RZ_LAUNCH_CHECK();
                 e->mcts_launches++;
             } else {
-                RZ_TRY(net_forward_counted(e->nets[net], e->dp.batch_own + row0, e->dp.batch_enemy + row0, e->dp.policy + row0 * 64,
-                                           e->dp.value + row0, count, rows, e->cfg.net_impl, st));
+                RZ_TRY(net_forward(e->nets[net], e->dp.batch_own + row0, e->dp.batch_enemy + row0, e->dp.policy + row0 * 64,
+                                   e->dp.value + row0, rows, count, e->cfg.net_impl, st, nullptr));
                 e->nn_launches++;
             }
         }

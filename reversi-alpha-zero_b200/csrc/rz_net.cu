@@ -1,9 +1,11 @@
 // rz_net.cu -- network object: creation, weight loading (BN folding, wgmma packing), the generic
-// CUDA-core forward kernel (any ModelConfig, e.g. config/mini.yml's 16 filters x 1 block) and the
+// CUDA-core forward kernel (any ModelConfig, e.g. config/mini.yml's 16 filters x 1 block), the host
+// sequence of every tensor-core tower launch, the choice between implementations (net_forward) and the
 // predict entry points of the C ABI (agent/api.py:30-45 ReversiModelAPI.predict).
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
+#include <mutex>
 #include <new>
 #include "rz_bitboard.cuh"
 #include "rz_net.cuh"
@@ -150,8 +152,8 @@ __global__ void __launch_bounds__(kGThreads) net_generic_kernel(const float* __r
     }
 }
 
-int net_forward_generic(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value, size_t n,
-                        cudaStream_t stream, const uint32_t* n_dev) {
+static int net_forward_generic(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value, size_t n,
+                               cudaStream_t stream, const uint32_t* n_dev) {
     const int F = net->cfg.filters, V = net->cfg.value_fc;
     RZ_REQUIRE(F >= 2 && F <= 256, "generic kernel supports 2 <= filters <= 256 (got %d)", F);
     const size_t smem = ((size_t)2 * F * 100 + 128 + 64 + (V > 64 ? V : 64)) * sizeof(float);
@@ -177,6 +179,103 @@ int net_forward_generic(rz_net* net, const uint64_t* own, const uint64_t* enemy,
     return RZ_OK;
 }
 
+// ---- wgmma weight images -----------------------------------------------------------------------------
+static bool tc_width(int filters) { return filters == 64 || filters == 128 || filters == 256; }
+
+// tc_w0: [4 kc][F n][8 j], K index k = 8 kc + j = (kh*3+kw)*2 + c of conv0.kernel[kh][kw][c][n], zero for k >= 18
+template <int F>
+__global__ void pack_tc_w0_kernel(const float* __restrict__ k0, __half* __restrict__ out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= 4 * F * 8) return;
+    const int j = i & 7, n = (i >> 3) % F, kc = i / (8 * F), k = kc * 8 + j;
+    out[i] = __float2half_rn(k < 18 ? k0[(size_t)k * F + n] : 0.f);
+}
+// tc_w: [layer][tap][F/8 kc][F n][8 j] of kernel[tap][ci = 8 kc + j][n]; the towers stream it in stages of consecutive kc
+template <int F>
+__global__ void pack_tc_w_kernel(const float* __restrict__ blob, size_t off_res0, size_t stride, int n_layers, __half* __restrict__ out) {
+    const size_t total = (size_t)n_layers * 9 * F * F;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const int j = i & 7, n = (int)((i >> 3) % F), kc = (int)((i / (8 * F)) % (F / 8));
+        const size_t lt = i / ((size_t)F * F);
+        const int tap = (int)(lt % 9), l = (int)(lt / 9), ci = kc * 8 + j;
+        out[i] = __float2half_rn(blob[off_res0 + (size_t)l * stride + ((size_t)tap * F + ci) * F + n]);
+    }
+}
+
+template <int F>
+static int pack_tc(rz_net* net, cudaStream_t stream) {
+    pack_tc_w0_kernel<F><<<(4 * F * 8 + 255) / 256, 256, 0, stream>>>(net->blob + net->off_conv0, net->tc_w0);
+    if (net->cfg.res_blocks > 0)
+        pack_tc_w_kernel<F><<<num_sms() * 8, 256, 0, stream>>>(net->blob, net->off_res0, net->res_stride_conv, 2 * net->cfg.res_blocks, net->tc_w);
+    RZ_LAUNCH_CHECK();
+    return RZ_OK;
+}
+
+static int net_pack_tc(rz_net* net, cudaStream_t stream) {
+    switch (net->cfg.filters) {
+        case 64: return pack_tc<64>(net, stream);
+        case 128: return pack_tc<128>(net, stream);
+        default: return pack_tc<256>(net, stream);
+    }
+}
+
+// ---- tensor-core towers ------------------------------------------------------------------------------
+// The towers' launches on a network hold this lock: they share its residual scratch, head-feature buffer and res_done.
+// The launches' one-time setup (kernel attributes, CTA-pair occupancy) runs under it too.
+static std::mutex tower_mutex;
+
+// grows net->feat to at least n rows (under tower_mutex; a reallocation synchronises the device first, since launches on
+// other streams may still read the old buffer)
+static int head_features(rz_net* net, size_t n) {
+    if (n <= net->feat_rows) return RZ_OK;
+    RZ_CUDA_TRY(cudaDeviceSynchronize());
+    RZ_CUDA_TRY(cudaFree(net->feat));
+    net->feat = nullptr;
+    net->feat_rows = 0;
+    RZ_CUDA_TRY(cudaMalloc(&net->feat, n * kHeadFeatures * sizeof(float)));
+    net->feat_rows = n;
+    return RZ_OK;
+}
+
+static tc::Params tower_params(const rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value, size_t n,
+                               const uint32_t* n_dev, const TowerDebug* debug) {
+    tc::Params p;
+    p.w0 = net->tc_w0; p.w = net->tc_w; p.ss = net->scale_shift; p.blob = net->blob;
+    p.off_policy_conv = net->off_policy_conv; p.off_policy_fc_k = net->off_policy_fc_k; p.off_policy_fc_b = net->off_policy_fc_b;
+    p.off_value_conv = net->off_value_conv; p.off_value_fc1_k = net->off_value_fc1_k; p.off_value_fc1_b = net->off_value_fc1_b;
+    p.off_value_fc2_k = net->off_value_fc2_k; p.off_value_fc2_b = net->off_value_fc2_b;
+    p.own = own; p.enemy = enemy; p.policy = policy; p.value = value;
+    p.res = net->res; p.feat = net->feat;
+    p.dbg_tower = debug ? debug->tower : nullptr;
+    p.dbg_logits = debug ? debug->logits : nullptr;
+    p.dbg_vlogit = debug ? debug->vlogit : nullptr;
+    p.n = (uint32_t)n; p.n_dev = n_dev; p.n_layers = n_conv_layers(net->cfg); p.V = net->cfg.value_fc;
+    return p;
+}
+
+// one tower launch of n > 0 positions (the batch capacity when n_dev is set): the throughput tower of the network's width
+// (TCGEN05) or the split tower (SPLIT), then the batched dense heads
+static int tower_forward(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value, size_t n,
+                         const uint32_t* n_dev, int impl, cudaStream_t stream, const TowerDebug* debug) {
+    const int F = net->cfg.filters;
+    const bool split = impl == RZ_NET_IMPL_SPLIT;
+    if (split) RZ_REQUIRE(F == 256, "the split tower requires filters == 256 (got %d)", F);
+    else RZ_REQUIRE(tc_width(F), "the tensor-core tower requires filters 64, 128 or 256 (got %d)", F);
+    RZ_REQUIRE(net->cfg.value_fc <= (int)tc::kTcMaxV, "the tensor-core tower supports value_fc_size <= %u", tc::kTcMaxV);
+    RZ_REQUIRE(n < (split ? 1ull << 27 : 1ull << 31), "batch too large");
+    std::lock_guard<std::mutex> lock(tower_mutex);
+    RZ_TRY(head_features(net, n));
+    const tc::Params p = tower_params(net, own, enemy, policy, value, n, n_dev, debug);
+    RZ_CUDA_TRY(cudaStreamWaitEvent(stream, net->res_done, 0));   // the previous launch on this scratch, whatever its stream
+    if (split) RZ_TRY(tc::launch_tower_split(p, stream));
+    else if (F == 256) RZ_TRY(tc::launch_tower(p, stream));
+    else RZ_TRY(tc::launch_tower_narrow(p, F, stream));
+    RZ_TRY(net_heads(p, stream));
+    RZ_CUDA_TRY(cudaEventRecord(net->res_done, stream));
+    return RZ_OK;
+}
+
+// ---- dispatch ----------------------------------------------------------------------------------------
 // Largest batch (capacity) for which AUTO runs the split tower; both towers compute the same bits.  0: on a 400 W H100
 // 80GB HBM3 the split tower was not faster at any batch (ch5, n = 1..16: 0.50 ms vs 0.49-0.50 ms per launch; n = 32:
 // 0.99 vs 0.50 ms), tools/search_latency_bench.py, DESIGN.md §5 "Split tower".
@@ -185,37 +284,23 @@ constexpr size_t kSplitMaxBatch = 0;
 // AUTO: the wgmma tower for every width it has (64, 128, 256 filters) and value heads it holds; the generic fp32 kernel
 // for everything else.  The narrow tower was faster than the generic kernel at every batch size measured (DESIGN.md §6
 // "Narrow towers"), so it has no batch threshold.
-int select_impl(const rz_net* net, size_t n, int impl) {
+static int select_impl(const rz_net* net, size_t n, int impl) {
     if (impl != RZ_NET_IMPL_AUTO) return impl;
     if (!tc_width(net->cfg.filters) || net->cfg.value_fc > (int)tc::kTcMaxV) return RZ_NET_IMPL_GENERIC;
     if (net->cfg.filters != 256) return RZ_NET_IMPL_TCGEN05;
     return n <= kSplitMaxBatch ? RZ_NET_IMPL_SPLIT : RZ_NET_IMPL_TCGEN05;
 }
 
-int net_forward(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value, size_t n, int impl,
-                cudaStream_t stream) {
+int net_forward(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value, size_t n,
+                const uint32_t* n_dev, int impl, cudaStream_t stream, const TowerDebug* debug) {
     if (!net->loaded) { set_error("rz_net: weights not loaded"); return RZ_ESTATE; }
     if (n == 0) return RZ_OK;
     impl = select_impl(net, n, impl);
-    if (impl == RZ_NET_IMPL_TCGEN05 || impl == RZ_NET_IMPL_SPLIT) {
-        if (impl == RZ_NET_IMPL_SPLIT) {
-            RZ_REQUIRE(net->cfg.filters == 256, "the split tower requires filters == 256 (got %d)", net->cfg.filters);
-            return net_forward_split(net, own, enemy, policy, value, n, stream, nullptr);
-        }
-        RZ_REQUIRE(tc_width(net->cfg.filters), "the tensor-core tower requires filters 64, 128 or 256 (got %d)", net->cfg.filters);
-        return net_forward_tc(net, own, enemy, policy, value, n, stream, nullptr);
-    }
+    if (impl == RZ_NET_IMPL_TCGEN05 || impl == RZ_NET_IMPL_SPLIT)
+        return tower_forward(net, own, enemy, policy, value, n, n_dev, impl, stream, debug);
+    RZ_REQUIRE(!debug, "rz_net_debug_heads_impl_dev: impl must be AUTO, TCGEN05 or SPLIT (got %d)", impl);
     RZ_REQUIRE(impl == RZ_NET_IMPL_GENERIC, "unknown net impl %d", impl);
-    return net_forward_generic(net, own, enemy, policy, value, n, stream);
-}
-
-int net_forward_counted(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value,
-                        const uint32_t* count_dev, size_t max_n, int impl, cudaStream_t stream) {
-    if (!net->loaded) { set_error("rz_net: weights not loaded"); return RZ_ESTATE; }
-    impl = select_impl(net, max_n, impl);
-    if (impl == RZ_NET_IMPL_TCGEN05) return net_forward_tc(net, own, enemy, policy, value, max_n, stream, nullptr, count_dev);
-    if (impl == RZ_NET_IMPL_SPLIT) return net_forward_split(net, own, enemy, policy, value, max_n, stream, nullptr, count_dev);
-    return net_forward_generic(net, own, enemy, policy, value, max_n, stream, count_dev);
+    return net_forward_generic(net, own, enemy, policy, value, n, stream, n_dev);
 }
 
 static int finish_load(rz_net* net, cudaStream_t stream) {
@@ -231,8 +316,7 @@ static int finish_load(rz_net* net, cudaStream_t stream) {
     fold_bn_kernel<<<1, 32, 0, stream>>>(net->blob, net->off_policy_conv, (size_t)F * 2, 2, ssh, ssh + 2);
     fold_bn_kernel<<<1, 32, 0, stream>>>(net->blob, net->off_value_conv, (size_t)F, 1, ssh + 4, ssh + 5);
     RZ_LAUNCH_CHECK();
-    if (F == 256) RZ_TRY(net_pack_tc(net, stream));
-    else if (tc_width(F)) RZ_TRY(net_pack_tc_narrow(net, stream));
+    if (tc_width(F)) RZ_TRY(net_pack_tc(net, stream));
     RZ_CUDA_TRY(cudaStreamSynchronize(stream));
     net->loaded = true;
     net->weights_version++;
@@ -325,41 +409,34 @@ int rz_net_set_tower_cluster(int cluster) { return set_tower_cluster(cluster); }
 int rz_net_predict_dev(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value, size_t n, int impl,
                        void* stream) {
     RZ_REQUIRE(net && (n == 0 || (own && enemy && policy && value)), "rz_net_predict_dev: null pointer");
-    return net_forward(net, own, enemy, policy, value, n, impl, (cudaStream_t)stream);
+    return net_forward(net, own, enemy, policy, value, n, nullptr, impl, (cudaStream_t)stream, nullptr);
 }
 
 int rz_net_predict_counted_dev(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value,
                                const uint32_t* count_dev, size_t max_n, int impl, void* stream) {
     RZ_REQUIRE(net && count_dev && (max_n == 0 || (own && enemy && policy && value)), "rz_net_predict_counted_dev: null pointer");
-    if (max_n == 0) return RZ_OK;
-    return net_forward_counted(net, own, enemy, policy, value, count_dev, max_n, impl, (cudaStream_t)stream);
+    return net_forward(net, own, enemy, policy, value, max_n, count_dev, impl, (cudaStream_t)stream, nullptr);
 }
 
 int rz_net_debug_tower_dev(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value, float* tower, size_t n,
                            void* stream) {
     RZ_REQUIRE(net && own && enemy && policy && value && tower, "rz_net_debug_tower_dev: null pointer");
-    if (!net->loaded) { set_error("rz_net: weights not loaded"); return RZ_ESTATE; }
-    return net_forward_tc(net, own, enemy, policy, value, n, (cudaStream_t)stream, tower);
+    const TowerDebug debug = {tower, nullptr, nullptr};
+    return net_forward(net, own, enemy, policy, value, n, nullptr, RZ_NET_IMPL_TCGEN05, (cudaStream_t)stream, &debug);
 }
 
 int rz_net_debug_heads_dev(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value, float* tower,
                            float* policy_logits, float* value_logit, size_t n, void* stream) {
     RZ_REQUIRE(net && own && enemy && policy && value && policy_logits && value_logit, "rz_net_debug_heads_dev: null pointer");
-    if (!net->loaded) { set_error("rz_net: weights not loaded"); return RZ_ESTATE; }
-    return net_forward_tc(net, own, enemy, policy, value, n, (cudaStream_t)stream, tower, nullptr, policy_logits, value_logit);
+    const TowerDebug debug = {tower, policy_logits, value_logit};
+    return net_forward(net, own, enemy, policy, value, n, nullptr, RZ_NET_IMPL_TCGEN05, (cudaStream_t)stream, &debug);
 }
 
 int rz_net_debug_heads_impl_dev(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value, float* tower,
                                 float* policy_logits, float* value_logit, size_t n, int impl, void* stream) {
     RZ_REQUIRE(net && own && enemy && policy && value && policy_logits && value_logit, "rz_net_debug_heads_impl_dev: null pointer");
-    if (!net->loaded) { set_error("rz_net: weights not loaded"); return RZ_ESTATE; }
-    RZ_REQUIRE(tc_width(net->cfg.filters), "the tensor-core tower requires filters 64, 128 or 256 (got %d)", net->cfg.filters);
-    if (n == 0) return RZ_OK;
-    impl = select_impl(net, n, impl);
-    if (impl == RZ_NET_IMPL_SPLIT)
-        return net_forward_split(net, own, enemy, policy, value, n, (cudaStream_t)stream, tower, nullptr, policy_logits, value_logit);
-    RZ_REQUIRE(impl == RZ_NET_IMPL_TCGEN05, "rz_net_debug_heads_impl_dev: impl must be AUTO, TCGEN05 or SPLIT (got %d)", impl);
-    return net_forward_tc(net, own, enemy, policy, value, n, (cudaStream_t)stream, tower, nullptr, policy_logits, value_logit);
+    const TowerDebug debug = {tower, policy_logits, value_logit};
+    return net_forward(net, own, enemy, policy, value, n, nullptr, impl, (cudaStream_t)stream, &debug);
 }
 
 int rz_net_select_impl(const rz_net* net, size_t n, int* impl) {
@@ -393,7 +470,7 @@ int rz_net_predict(rz_net* net, const uint8_t* planes, float* policy, float* val
     float* d_val = d_pol + n * 64;
     cudaError_t ce = cudaMemcpyAsync(d_own, hb, n * 16, cudaMemcpyHostToDevice, 0);
     int rc = RZ_OK;
-    if (ce == cudaSuccess) rc = net_forward(net, d_own, d_en, d_pol, d_val, n, impl, 0);
+    if (ce == cudaSuccess) rc = net_forward(net, d_own, d_en, d_pol, d_val, n, nullptr, impl, 0, nullptr);
     if (ce == cudaSuccess && rc == RZ_OK) ce = cudaMemcpyAsync(policy, d_pol, n * 64 * sizeof(float), cudaMemcpyDeviceToHost, 0);
     if (ce == cudaSuccess && rc == RZ_OK) ce = cudaMemcpyAsync(value, d_val, n * sizeof(float), cudaMemcpyDeviceToHost, 0);
     if (ce == cudaSuccess && rc == RZ_OK) ce = cudaStreamSynchronize(0);

@@ -8,7 +8,6 @@
 //   scale = gamma / sqrt(var + 1e-3),  shift = beta + (bias - mean) * scale.
 #pragma once
 #include <cuda_fp16.h>
-#include <mutex>
 #include "rz_common.cuh"
 
 struct rz_net {
@@ -25,8 +24,8 @@ struct rz_net {
     size_t off_value_conv, off_value_fc1_k, off_value_fc1_b, off_value_fc2_k, off_value_fc2_b;
     // wgmma tower (F == 64, 128 or 256)
     __half* tc_w0;       // [4 kc][F n][8] fp16: layer-0 weights, K = 18 padded to 32, K-major no-swizzle image
-    __half* tc_w;        // F = 256: [2R layers][36 stages][8 kc][256 n][8] fp16, one 32 KB shared-memory image per pipeline stage;
-                         // F = 64 / 128: [2R layers][9 taps][F/8 kc][F n][8] fp16, a stage is 3 / 1 consecutive taps
+    __half* tc_w;        // [2R layers][9 taps][F/8 kc][F n][8] fp16: input channel ci = 8 kc + j; a weight stage is a run of
+                         // consecutive kc: F = 256: 8 kc (64 input channels of one tap, 32 KB); 128: one tap; 64: three taps
     // fp32 residual-stream scratch of the tower kernel ([CTA][kTowerResFloatsPerCta]); launches from different streams
     // are ordered through res_done, recorded after every launch that uses it
     float* res;
@@ -49,37 +48,19 @@ inline int n_conv_layers(const rz_net_cfg& c) { return 1 + 2 * c.res_blocks; }
 // per-layer folded BN parameters: scale at [l][0][*], shift at [l][1][*]
 inline size_t ss_floats(const rz_net_cfg& c) { return (size_t)n_conv_layers(c) * 2 * c.filters + 4 + 2; }
 
-int net_forward_generic(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value, size_t n,
-                        cudaStream_t stream, const uint32_t* n_dev = nullptr);
-// batch size known only on the device (count_dev), at most max_n
-int net_forward_counted(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value,
-                        const uint32_t* count_dev, size_t max_n, int impl, cudaStream_t stream);
-// the wgmma tower for F = 256 (rz_net_tc.cu) and, through net_forward_tc_narrow, F = 64 and 128
-int net_forward_tc(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value, size_t n,
-                   cudaStream_t stream, float* dbg_tower /* nullable: [n][64][F] fp32 tower output */,
-                   const uint32_t* n_dev = nullptr /* nullable: actual batch size in device memory (<= n) */,
-                   float* dbg_logits = nullptr /* nullable: [n][64] policy logits */, float* dbg_vlogit = nullptr /* nullable: [n] */);
-// same function as net_forward_tc, bit for bit, one 8-CTA cluster per 2-board tile (small batches, rz_net_split.cu)
-int net_forward_split(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value, size_t n,
-                      cudaStream_t stream, float* dbg_tower, const uint32_t* n_dev = nullptr, float* dbg_logits = nullptr,
-                      float* dbg_vlogit = nullptr);
-// RZ_NET_IMPL_AUTO -> the implementation used for a batch of capacity n
-int select_impl(const rz_net* net, size_t n, int impl);
-int net_pack_tc(rz_net* net, cudaStream_t stream);
-// the wgmma towers' launches on a network hold this lock: they share its residual scratch and head-feature buffer
-std::mutex& tower_mutex();
-// grows net->feat to at least n rows (under tower_mutex(); a reallocation synchronises the device first, since launches on
-// other streams may still read the old buffer)
-int head_features(rz_net* net, size_t n);
-// the same tower for 64 and 128 filters, B = 512 / F boards per tile (rz_net_tc_narrow.cu)
-int net_forward_tc_narrow(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value, size_t n,
-                          cudaStream_t stream, float* dbg_tower, const uint32_t* n_dev, float* dbg_logits, float* dbg_vlogit);
-int net_pack_tc_narrow(rz_net* net, cudaStream_t stream);
-inline bool tc_width(int filters) { return filters == 64 || filters == 128 || filters == 256; }
-// thread-block clusters of the tower kernels: 2 = CTA pairs sharing the weight stages (default), 1 = single CTAs
+// optional outputs of the tensor-core towers, each nullable: fp32 tower output [n][64 pixels][F], policy logits [n][64]
+// (before the softmax), value logit [n] (before the tanh)
+struct TowerDebug {
+    float* tower;
+    float* logits;
+    float* vlogit;
+};
+// policy [n][64] and value [n] of n positions (*n_dev of them when n_dev is set: a count known only on the device, <= n)
+// by implementation impl (RZ_NET_IMPL_*; AUTO picks by n), on stream; debug needs a tensor-core tower
+int net_forward(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value, size_t n,
+                const uint32_t* n_dev, int impl, cudaStream_t stream, const TowerDebug* debug);
+// thread-block clusters of the throughput towers: 2 = CTA pairs sharing the weight stages (default), 1 = single CTAs
 int set_tower_cluster(int cluster);
 int tower_cluster();   // the current setting: rz_net_set_tower_cluster, else RZ_TOWER_CLUSTER, else 2
-int net_forward(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value, size_t n, int impl,
-                cudaStream_t stream);
 
 }  // namespace rz

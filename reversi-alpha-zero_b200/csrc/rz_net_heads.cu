@@ -128,22 +128,6 @@ static_assert(kBoards == 4, "the feature tile is read as one float4 per feature"
 
 }  // namespace heads
 
-std::mutex& tower_mutex() {
-    static std::mutex m;
-    return m;
-}
-
-int head_features(rz_net* net, size_t n) {
-    if (n <= net->feat_rows) return RZ_OK;
-    RZ_CUDA_TRY(cudaDeviceSynchronize());   // launches on any stream may still use the old buffer
-    RZ_CUDA_TRY(cudaFree(net->feat));
-    net->feat = nullptr;
-    net->feat_rows = 0;
-    RZ_CUDA_TRY(cudaMalloc(&net->feat, n * kHeadFeatures * sizeof(float)));
-    net->feat_rows = n;
-    return RZ_OK;
-}
-
 int net_heads(const tc::Params& p, cudaStream_t stream) {
     static bool attr = false;
     if (!attr) {

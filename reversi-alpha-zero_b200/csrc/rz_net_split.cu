@@ -16,6 +16,8 @@
 //   * head features: the fp32 tower output of the tile is gathered into CTA 0 (over the then idle operand buffer and weight
 //     ring), whose threads repeat the head sums of net_tower_kernel in its order (per lane over i = 0..31, then the lane
 //     quad) and store the same head features; the dense heads run afterwards in the batched head pass (rz_net_heads.cu).
+// Host side: launch_tower_split, one 8-CTA cluster (__cluster_dims__) per tile of the batch capacity, called by the tower
+// sequence in rz_net.cu (RZ_NET_IMPL_SPLIT).
 #include "rz_bitboard.cuh"
 #include "rz_net.cuh"
 #include "rz_tc_common.cuh"
@@ -246,35 +248,15 @@ __global__ void __cluster_dims__(kCluster, 1, 1) __launch_bounds__(kThreads, 1) 
 
 }  // namespace split
 
-int net_forward_split(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value, size_t n, cudaStream_t stream,
-                      float* dbg_tower, const uint32_t* n_dev, float* dbg_logits, float* dbg_vlogit) {
-    RZ_REQUIRE(net->cfg.filters == 256, "split tower requires 256 filters");
-    RZ_REQUIRE(net->cfg.value_fc <= (int)tc::kTcMaxV, "split tower supports value_fc_size <= %u", tc::kTcMaxV);
-    RZ_REQUIRE(n < (1ull << 27), "batch too large");
+int tc::launch_tower_split(const Params& p, cudaStream_t stream) {
     static bool attr = false;
     if (!attr) {
         RZ_CUDA_TRY(cudaFuncSetAttribute(split::net_split_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)split::kSmemAlloc));
         attr = true;
     }
-    tc::Params p;
-    p.w0 = net->tc_w0; p.w = net->tc_w; p.ss = net->scale_shift; p.blob = net->blob;
-    p.off_policy_conv = net->off_policy_conv; p.off_policy_fc_k = net->off_policy_fc_k; p.off_policy_fc_b = net->off_policy_fc_b;
-    p.off_value_conv = net->off_value_conv; p.off_value_fc1_k = net->off_value_fc1_k; p.off_value_fc1_b = net->off_value_fc1_b;
-    p.off_value_fc2_k = net->off_value_fc2_k; p.off_value_fc2_b = net->off_value_fc2_b;
-    p.own = own; p.enemy = enemy; p.policy = policy; p.value = value; p.dbg_tower = dbg_tower;
-    p.dbg_logits = dbg_logits; p.dbg_vlogit = dbg_vlogit;
-    p.n = (uint32_t)n; p.n_dev = n_dev; p.n_layers = 1 + 2 * net->cfg.res_blocks; p.V = net->cfg.value_fc;
-    p.res = nullptr;
-    const uint32_t ntiles = (uint32_t)((n + 1) / 2);
-    if (ntiles == 0) return RZ_OK;
-    std::lock_guard<std::mutex> lock(tower_mutex());
-    RZ_TRY(head_features(net, n));
-    p.feat = net->feat;
-    RZ_CUDA_TRY(cudaStreamWaitEvent(stream, net->res_done, 0));   // the previous launch on the head-feature buffer
+    const uint32_t ntiles = (p.n + 1) / 2;
     split::net_split_kernel<<<ntiles * split::kCluster, split::kThreads, split::kSmemAlloc, stream>>>(p);
     RZ_LAUNCH_CHECK();
-    RZ_TRY(net_heads(p, stream));
-    RZ_CUDA_TRY(cudaEventRecord(net->res_done, stream));
     return RZ_OK;
 }
 

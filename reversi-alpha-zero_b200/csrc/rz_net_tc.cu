@@ -30,8 +30,9 @@
 //     all boards (rz_net_heads.cu) instead of once per tile on the math warps.
 // Global traffic per position: 16 B in and 768 B of head features out (the head pass reads them back and writes the
 // 260 B of policy and value).  Algorithmic work: 2 * 755,343,616 flop (SURVEY 3.2).
+// Host side: launch_tower, a CTA-pair launch (launch_tower_pairs, rz_tc_common.cuh) called by the one tower sequence of
+// all three tower families (tower_forward, rz_net.cu).  rz_net.cu also packs the weight image at load (tc_w, rz_net.cuh).
 #include <stdlib.h>
-#include <mutex>
 #include <type_traits>
 #include "rz_bitboard.cuh"
 #include "rz_net.cuh"
@@ -40,10 +41,9 @@
 namespace rz {
 namespace tc {
 
-// warps 0..7 = two math warpgroups, warps 8..11 = producer warpgroup (one thread streams the weights).  Registers are
-// handed from the producer warpgroup to the math warpgroups (setmaxnreg): the math threads hold a 64 x 256 fp32
-// accumulator (128 registers) each.
-constexpr int kThreads = 384;
+// kThreads = 384: warps 0..7 = two math warpgroups, warps 8..11 = producer warpgroup (one thread streams the weights).
+// Registers are handed from the producer warpgroup to the math warpgroups (setmaxnreg): the math threads hold a 64 x 256
+// fp32 accumulator (128 registers) each.
 constexpr uint32_t kProducerRegs = 40, kMathRegs = 232;
 constexpr int kMathThreads = 256;
 constexpr uint32_t kActCg = 2896, kActSlot = 144;
@@ -378,34 +378,11 @@ __global__ void __launch_bounds__(kThreads, 1) net_tower_kernel(const Params pp)
     if (CL > 1) cluster_sync_all();  // no CTA leaves while a peer may still multicast into it / arrive on its barriers
 }
 
-// ---- weight packing -----------------------------------------------------------------------------------
-__global__ void pack_w0_kernel(const float* __restrict__ k0, __half* __restrict__ out) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;  // over [4 kc][256 n][8 j]
-    if (i >= 4 * 256 * 8) return;
-    const int j = i & 7, n = (i >> 3) & 255, kc = i >> 11, k = kc * 8 + j;
-    // conv0.kernel[kh][kw][c][n], K index = (kh*3+kw)*2 + c
-    out[i] = __float2half_rn(k < 18 ? k0[(size_t)k * 256 + n] : 0.f);
-}
-__global__ void pack_w_kernel(const float* __restrict__ blob, size_t off_res0, size_t stride, int n_layers, __half* __restrict__ out) {
-    const size_t total = (size_t)n_layers * 36 * 8 * 256 * 8;
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-        const int j = i & 7, n = (i >> 3) & 255, kc = (i >> 11) & 7;
-        const size_t ls = i >> 14;
-        const int s = (int)(ls % 36), l = (int)(ls / 36);
-        const int tap = s >> 2, kb = s & 3, ci = kb * 64 + kc * 8 + j;
-        out[i] = __float2half_rn(blob[off_res0 + (size_t)l * stride + ((size_t)tap * 256 + ci) * 256 + n]);
-    }
+int launch_tower(const Params& p, cudaStream_t stream) {
+    return launch_tower_pairs<net_tower_kernel<1>, net_tower_kernel<2>, kSmemAlloc, 2>(p, stream);
 }
 
 }  // namespace tc
-
-int net_pack_tc(rz_net* net, cudaStream_t stream) {
-    tc::pack_w0_kernel<<<(4 * 256 * 8 + 255) / 256, 256, 0, stream>>>(net->blob + net->off_conv0, net->tc_w0);
-    if (net->cfg.res_blocks > 0)
-        tc::pack_w_kernel<<<num_sms() * 8, 256, 0, stream>>>(net->blob, net->off_res0, net->res_stride_conv, 2 * net->cfg.res_blocks, net->tc_w);
-    RZ_LAUNCH_CHECK();
-    return RZ_OK;
-}
 
 static int g_cluster = 0;        // 0: not yet decided (RZ_TOWER_CLUSTER, default 2)
 
@@ -421,61 +398,6 @@ int tower_cluster() {
         g_cluster = (cs && atoi(cs) == 1) ? 1 : 2;
     }
     return g_cluster;
-}
-
-int net_forward_tc(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value, size_t n, cudaStream_t stream,
-                   float* dbg_tower, const uint32_t* n_dev, float* dbg_logits, float* dbg_vlogit) {
-    if (net->cfg.filters == 64 || net->cfg.filters == 128)
-        return net_forward_tc_narrow(net, own, enemy, policy, value, n, stream, dbg_tower, n_dev, dbg_logits, dbg_vlogit);
-    RZ_REQUIRE(net->cfg.filters == 256, "wgmma tower requires 64, 128 or 256 filters (got %d)", net->cfg.filters);
-    RZ_REQUIRE(net->cfg.value_fc <= (int)tc::kTcMaxV, "wgmma tower supports value_fc_size <= %u", tc::kTcMaxV);
-    RZ_REQUIRE(n < (1ull << 31), "batch too large");
-    static int max_pairs = -1;
-    if (max_pairs < 0) {
-        RZ_CUDA_TRY(cudaFuncSetAttribute(tc::net_tower_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc::kSmemAlloc));
-        RZ_CUDA_TRY(cudaFuncSetAttribute(tc::net_tower_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc::kSmemAlloc));
-        // how many CTA pairs can be resident at once: an SM without a free partner in its GPC cannot take a pair
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3((unsigned)num_sms() & ~1u); cfg.blockDim = dim3(tc::kThreads); cfg.dynamicSmemBytes = tc::kSmemAlloc;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr; cfg.numAttrs = 1;
-        RZ_CUDA_TRY(cudaOccupancyMaxActiveClusters(&max_pairs, tc::net_tower_kernel<2>, &cfg));
-    }
-    const int cluster = tower_cluster() == 2 && max_pairs >= 1 ? 2 : 1;
-    tc::Params p;
-    p.w0 = net->tc_w0; p.w = net->tc_w; p.ss = net->scale_shift; p.blob = net->blob;
-    p.off_policy_conv = net->off_policy_conv; p.off_policy_fc_k = net->off_policy_fc_k; p.off_policy_fc_b = net->off_policy_fc_b;
-    p.off_value_conv = net->off_value_conv; p.off_value_fc1_k = net->off_value_fc1_k; p.off_value_fc1_b = net->off_value_fc1_b;
-    p.off_value_fc2_k = net->off_value_fc2_k; p.off_value_fc2_b = net->off_value_fc2_b;
-    p.own = own; p.enemy = enemy; p.policy = policy; p.value = value; p.dbg_tower = dbg_tower;
-    p.dbg_logits = dbg_logits; p.dbg_vlogit = dbg_vlogit;
-    p.n = (uint32_t)n; p.n_dev = n_dev; p.n_layers = 1 + 2 * net->cfg.res_blocks; p.V = net->cfg.value_fc;
-    p.res = net->res;
-    std::lock_guard<std::mutex> lock(tower_mutex());
-    RZ_TRY(head_features(net, n));
-    p.feat = net->feat;
-    RZ_CUDA_TRY(cudaStreamWaitEvent(stream, net->res_done, 0));   // the previous launch on this scratch, whatever its stream
-    const uint32_t ntiles = (uint32_t)((n + 1) / 2);
-    uint32_t grid = ntiles < (uint32_t)num_sms() ? ntiles : (uint32_t)num_sms();
-    if (cluster == 1) {
-        tc::net_tower_kernel<1><<<grid, tc::kThreads, tc::kSmemAlloc, stream>>>(p);
-    } else {
-        grid = (grid + 1) & ~1u;  // whole clusters; a surplus CTA runs dummy tiles
-        if (grid > 2u * (uint32_t)max_pairs) grid = 2u * (uint32_t)max_pairs;
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(grid); cfg.blockDim = dim3(tc::kThreads); cfg.dynamicSmemBytes = tc::kSmemAlloc; cfg.stream = stream;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr; cfg.numAttrs = 1;
-        RZ_CUDA_TRY(cudaLaunchKernelEx(&cfg, tc::net_tower_kernel<2>, p));
-    }
-    RZ_LAUNCH_CHECK();
-    RZ_TRY(net_heads(p, stream));
-    RZ_CUDA_TRY(cudaEventRecord(net->res_done, stream));
-    return RZ_OK;
 }
 
 }  // namespace rz

@@ -16,8 +16,9 @@
 //     head-conv sums are complete in its lane quad, so they need no cross-warpgroup partial-sum array.  The dense heads
 //     run afterwards as one batched pass (rz_net_heads.cu).
 // Every output element goes through the same operations whichever tile slot its board lands in.
-#include <stdlib.h>
-#include <mutex>
+// Host side: launch_tower_narrow, the CTA-pair launch of rz_net_tc.cu (launch_tower_pairs, rz_tc_common.cuh) with B-board
+// tiles, called by the tower sequence in rz_net.cu.  rz_net.cu also packs the weights at load, in the one layout of every
+// width (tc_w, rz_net.cuh).
 #include <type_traits>
 #include "rz_bitboard.cuh"
 #include "rz_net.cuh"
@@ -27,7 +28,6 @@ namespace rz {
 namespace tc {
 namespace narrow {
 
-constexpr int kThreads = 384;
 constexpr uint32_t kProducerRegs = 40, kMathRegs = 232;
 constexpr uint32_t kActSlot = 144;
 constexpr uint32_t kStages = 3;
@@ -347,100 +347,17 @@ __global__ void __launch_bounds__(kThreads, 1) net_tower_narrow_kernel(const Par
     if (CL > 1) cluster_sync_all();
 }
 
-// ---- weight packing -----------------------------------------------------------------------------------
-template <int F>
-__global__ void pack_w0_narrow_kernel(const float* __restrict__ k0, __half* __restrict__ out) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;   // over [4 kc][F n][8 j]
-    if (i >= 4 * F * 8) return;
-    const int j = i & 7, n = (i >> 3) % F, kc = i / (8 * F), k = kc * 8 + j;
-    out[i] = __float2half_rn(k < 18 ? k0[(size_t)k * F + n] : 0.f);   // conv0.kernel[kh][kw][c][n], K index = (kh*3+kw)*2 + c
-}
-// [layer][tap][F/8 kc][F n][8 j]: a stage is TPS consecutive taps
-template <int F>
-__global__ void pack_w_narrow_kernel(const float* __restrict__ blob, size_t off_res0, size_t stride, int n_layers, __half* __restrict__ out) {
-    const size_t total = (size_t)n_layers * 9 * F * F;
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-        const int j = i & 7, n = (int)((i >> 3) % F), kc = (int)((i / (8 * F)) % (F / 8));
-        const size_t lt = i / ((size_t)F * F);
-        const int tap = (int)(lt % 9), l = (int)(lt / 9), ci = kc * 8 + j;
-        out[i] = __float2half_rn(blob[off_res0 + (size_t)l * stride + ((size_t)tap * F + ci) * F + n]);
-    }
-}
-
-template <int F>
-int pack(rz_net* net, cudaStream_t stream) {
-    pack_w0_narrow_kernel<F><<<(4 * F * 8 + 255) / 256, 256, 0, stream>>>(net->blob + net->off_conv0, net->tc_w0);
-    if (net->cfg.res_blocks > 0)
-        pack_w_narrow_kernel<F><<<num_sms() * 8, 256, 0, stream>>>(net->blob, net->off_res0, net->res_stride_conv, 2 * net->cfg.res_blocks, net->tc_w);
-    RZ_LAUNCH_CHECK();
-    return RZ_OK;
-}
-
-template <int F>
-int launch(const Params& p, size_t n, cudaStream_t stream) {
-    using C = Cfg<F>;
-    static int max_pairs = -1;
-    if (max_pairs < 0) {
-        RZ_CUDA_TRY(cudaFuncSetAttribute(net_tower_narrow_kernel<F, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::kSmemAlloc));
-        RZ_CUDA_TRY(cudaFuncSetAttribute(net_tower_narrow_kernel<F, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::kSmemAlloc));
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3((unsigned)num_sms() & ~1u); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = C::kSmemAlloc;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr; cfg.numAttrs = 1;
-        RZ_CUDA_TRY(cudaOccupancyMaxActiveClusters(&max_pairs, net_tower_narrow_kernel<F, 2>, &cfg));
-    }
-    const int cluster = tower_cluster() == 2 && max_pairs >= 1 ? 2 : 1;
-    const uint32_t ntiles = (uint32_t)((n + C::B - 1) / C::B);
-    uint32_t grid = ntiles < (uint32_t)num_sms() ? ntiles : (uint32_t)num_sms();
-    if (cluster == 1) {
-        net_tower_narrow_kernel<F, 1><<<grid, kThreads, C::kSmemAlloc, stream>>>(p);
-    } else {
-        grid = (grid + 1) & ~1u;   // whole clusters; a surplus CTA runs dummy tiles
-        if (grid > 2u * (uint32_t)max_pairs) grid = 2u * (uint32_t)max_pairs;
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = C::kSmemAlloc; cfg.stream = stream;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr; cfg.numAttrs = 1;
-        RZ_CUDA_TRY(cudaLaunchKernelEx(&cfg, net_tower_narrow_kernel<F, 2>, p));
-    }
-    RZ_LAUNCH_CHECK();
-    return RZ_OK;
-}
-
 }  // namespace narrow
+
+int launch_tower_narrow(const Params& p, int filters, cudaStream_t stream) {
+    using narrow::Cfg;
+    using narrow::net_tower_narrow_kernel;
+    if (filters == 128)
+        return launch_tower_pairs<net_tower_narrow_kernel<128, 1>, net_tower_narrow_kernel<128, 2>, Cfg<128>::kSmemAlloc, Cfg<128>::B>(
+            p, stream);
+    return launch_tower_pairs<net_tower_narrow_kernel<64, 1>, net_tower_narrow_kernel<64, 2>, Cfg<64>::kSmemAlloc, Cfg<64>::B>(p, stream);
+}
+
 }  // namespace tc
-
-int net_pack_tc_narrow(rz_net* net, cudaStream_t stream) {
-    return net->cfg.filters == 128 ? tc::narrow::pack<128>(net, stream) : tc::narrow::pack<64>(net, stream);
-}
-
-int net_forward_tc_narrow(rz_net* net, const uint64_t* own, const uint64_t* enemy, float* policy, float* value, size_t n, cudaStream_t stream,
-                          float* dbg_tower, const uint32_t* n_dev, float* dbg_logits, float* dbg_vlogit) {
-    const int F = net->cfg.filters;
-    RZ_REQUIRE(F == 64 || F == 128, "narrow wgmma tower requires 64 or 128 filters (got %d)", F);
-    RZ_REQUIRE(net->cfg.value_fc <= (int)tc::kTcMaxV, "wgmma tower supports value_fc_size <= %u", tc::kTcMaxV);
-    RZ_REQUIRE(n < (1ull << 31), "batch too large");
-    tc::Params p;
-    p.w0 = net->tc_w0; p.w = net->tc_w; p.ss = net->scale_shift; p.blob = net->blob;
-    p.off_policy_conv = net->off_policy_conv; p.off_policy_fc_k = net->off_policy_fc_k; p.off_policy_fc_b = net->off_policy_fc_b;
-    p.off_value_conv = net->off_value_conv; p.off_value_fc1_k = net->off_value_fc1_k; p.off_value_fc1_b = net->off_value_fc1_b;
-    p.off_value_fc2_k = net->off_value_fc2_k; p.off_value_fc2_b = net->off_value_fc2_b;
-    p.own = own; p.enemy = enemy; p.policy = policy; p.value = value; p.dbg_tower = dbg_tower;
-    p.dbg_logits = dbg_logits; p.dbg_vlogit = dbg_vlogit;
-    p.n = (uint32_t)n; p.n_dev = n_dev; p.n_layers = 1 + 2 * net->cfg.res_blocks; p.V = net->cfg.value_fc;
-    p.res = net->res;
-    std::lock_guard<std::mutex> lock(tower_mutex());
-    RZ_TRY(head_features(net, n));
-    p.feat = net->feat;
-    RZ_CUDA_TRY(cudaStreamWaitEvent(stream, net->res_done, 0));   // the previous launch on this scratch, whatever its stream
-    RZ_TRY(F == 128 ? tc::narrow::launch<128>(p, n, stream) : tc::narrow::launch<64>(p, n, stream));
-    RZ_TRY(net_heads(p, stream));
-    RZ_CUDA_TRY(cudaEventRecord(net->res_done, stream));
-    return RZ_OK;
-}
 
 }  // namespace rz

@@ -1,5 +1,5 @@
 // rz_tc_common.cuh -- PTX wrappers (mbarrier, bulk copy with cluster multicast, wgmma) and the pieces of the fused
-// tower kernel (rz_net_tc.cu) that do not depend on its pipeline: parameter block, layer-0 operand, head features.
+// tower kernels that do not depend on their pipelines: parameter block, CTA-pair launch, layer-0 operand, head features.
 #pragma once
 #include <cuda_fp16.h>
 #include "rz_bitboard.cuh"
@@ -177,6 +177,55 @@ struct Params {
 };
 
 constexpr uint32_t kTcMaxV = 512;
+
+// threads of the throughput towers: warps 0..7 = two math warpgroups, warps 8..11 = producer warpgroup
+constexpr int kThreads = 384;
+
+// Launches a throughput tower over the tiles of p.n boards, kBoards per tile: K2 in CTA pairs that share every weight
+// stage (tower_cluster() == 2, where the GPU can hold a pair), else K1 in single CTAs.  grid = min(tiles, SMs); for pairs
+// it is rounded up to whole clusters (a surplus CTA runs dummy tiles) and capped at the pairs the GPU holds at once.
+// Callers hold the tower lock (rz_net.cu), which also guards the one-time setup.
+template <void (*K1)(Params), void (*K2)(Params), uint32_t kSmem, uint32_t kBoards>
+int launch_tower_pairs(const Params& p, cudaStream_t stream) {
+    static int max_pairs = -1;
+    if (max_pairs < 0) {
+        RZ_CUDA_TRY(cudaFuncSetAttribute(K1, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmem));
+        RZ_CUDA_TRY(cudaFuncSetAttribute(K2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmem));
+        // how many CTA pairs can be resident at once: an SM without a free partner in its GPC cannot take a pair
+        cudaLaunchConfig_t cfg = {};
+        cfg.gridDim = dim3((unsigned)num_sms() & ~1u); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = kSmem;
+        cudaLaunchAttribute attr[1];
+        attr[0].id = cudaLaunchAttributeClusterDimension;
+        attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+        cfg.attrs = attr; cfg.numAttrs = 1;
+        RZ_CUDA_TRY(cudaOccupancyMaxActiveClusters(&max_pairs, K2, &cfg));
+    }
+    const int cluster = tower_cluster() == 2 && max_pairs >= 1 ? 2 : 1;
+    const uint32_t ntiles = (p.n + kBoards - 1) / kBoards;
+    uint32_t grid = ntiles < (uint32_t)num_sms() ? ntiles : (uint32_t)num_sms();
+    if (cluster == 1) {
+        K1<<<grid, kThreads, kSmem, stream>>>(p);
+    } else {
+        grid = (grid + 1) & ~1u;
+        if (grid > 2u * (uint32_t)max_pairs) grid = 2u * (uint32_t)max_pairs;
+        cudaLaunchConfig_t cfg = {};
+        cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = kSmem; cfg.stream = stream;
+        cudaLaunchAttribute attr[1];
+        attr[0].id = cudaLaunchAttributeClusterDimension;
+        attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+        cfg.attrs = attr; cfg.numAttrs = 1;
+        RZ_CUDA_TRY(cudaLaunchKernelEx(&cfg, K2, p));
+    }
+    RZ_LAUNCH_CHECK();
+    return RZ_OK;
+}
+
+// the tower families' launches on p.n boards, under the tower lock: 256 filters in 2-board tiles (rz_net_tc.cu); 64 and
+// 128 filters in 512 / F-board tiles (rz_net_tc_narrow.cu); 256 filters with every 2-board tile on an 8-CTA cluster
+// (rz_net_split.cu)
+int launch_tower(const Params& p, cudaStream_t stream);
+int launch_tower_narrow(const Params& p, int filters, cudaStream_t stream);
+int launch_tower_split(const Params& p, cudaStream_t stream);
 
 // layer-0 operand (agent/model.py:30-33 first convolution as a GEMM): im2col of the two bit planes of one board row m =
 // (g, x), K index = tap * 2 + plane padded to 32, two of the four 8-wide K chunks (kc0, kc0 + 1) per calling thread;

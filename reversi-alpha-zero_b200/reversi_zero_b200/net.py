@@ -72,28 +72,25 @@ class Net:
                                                             C.c_void_p(count_t.data_ptr()), max_n, impl, stream_ptr),
                     "rz_net_predict_counted_dev")
 
+    def _debug_dev(self, fn, tensors, *tail):
+        """rz_net_debug_<fn>_dev(net, <device pointers of tensors (None: NULL)>, *tail)"""
+        name = f"rz_net_debug_{fn}_dev"
+        ptrs = [C.c_void_p(t.data_ptr()) if t is not None else None for t in tensors]
+        _cabi.check(getattr(_cabi.lib(), name)(self._h, *ptrs, *tail), name)
+
     def debug_tower_dev(self, own_t, enemy_t, policy_t, value_t, tower_t, n, stream_ptr=None):
         """tensor-core tower path that also writes the fp32 tower output: tower_t holds n * 64 * cnn_filter_num floats,
         [position][pixel y*8+x][channel]"""
-        _cabi.check(_cabi.lib().rz_net_debug_tower_dev(self._h, C.c_void_p(own_t.data_ptr()), C.c_void_p(enemy_t.data_ptr()),
-                                                        C.c_void_p(policy_t.data_ptr()), C.c_void_p(value_t.data_ptr()),
-                                                        C.c_void_p(tower_t.data_ptr()), n, stream_ptr), "rz_net_debug_tower_dev")
+        self._debug_dev("tower", (own_t, enemy_t, policy_t, value_t, tower_t), n, stream_ptr)
 
     def debug_heads_dev(self, own_t, enemy_t, policy_t, value_t, logits_t, vlogit_t, n, tower_t=None, stream_ptr=None):
         """tensor-core tower path with the head outputs before softmax / tanh (and optionally the fp32 tower output,
         sized as for debug_tower_dev)"""
-        _cabi.check(_cabi.lib().rz_net_debug_heads_dev(self._h, C.c_void_p(own_t.data_ptr()), C.c_void_p(enemy_t.data_ptr()),
-                                                        C.c_void_p(policy_t.data_ptr()), C.c_void_p(value_t.data_ptr()),
-                                                        C.c_void_p(tower_t.data_ptr()) if tower_t is not None else None,
-                                                        C.c_void_p(logits_t.data_ptr()), C.c_void_p(vlogit_t.data_ptr()), n, stream_ptr),
-                    "rz_net_debug_heads_dev")
+        self._debug_dev("heads", (own_t, enemy_t, policy_t, value_t, tower_t, logits_t, vlogit_t), n, stream_ptr)
 
     def debug_heads_impl_dev(self, own_t, enemy_t, policy_t, value_t, logits_t, vlogit_t, n, impl, tower_t=None, stream_ptr=None):
         """debug_heads_dev with the tower implementation chosen (IMPL_AUTO, IMPL_TCGEN05 or IMPL_SPLIT)"""
-        _cabi.check(_cabi.lib().rz_net_debug_heads_impl_dev(
-            self._h, C.c_void_p(own_t.data_ptr()), C.c_void_p(enemy_t.data_ptr()), C.c_void_p(policy_t.data_ptr()),
-            C.c_void_p(value_t.data_ptr()), C.c_void_p(tower_t.data_ptr()) if tower_t is not None else None,
-            C.c_void_p(logits_t.data_ptr()), C.c_void_p(vlogit_t.data_ptr()), n, int(impl), stream_ptr), "rz_net_debug_heads_impl_dev")
+        self._debug_dev("heads_impl", (own_t, enemy_t, policy_t, value_t, tower_t, logits_t, vlogit_t), n, int(impl), stream_ptr)
 
     def select_impl(self, n):
         """the implementation IMPL_AUTO runs for a batch of n positions"""

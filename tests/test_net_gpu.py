@@ -196,6 +196,12 @@ def test_tcgen05_matches_generic_on_device():
         torch.cuda.synchronize()
         outs.append((d_pol.cpu().numpy(), d_val.cpu().numpy()))
     assert np.abs(outs[0][0] - outs[1][0]).max() <= 1e-3 and np.abs(outs[0][1] - outs[1][1]).max() <= 1e-3
+    # an empty batch is a no-op on the debug entry points as on predict_dev: no launch, nothing written
+    pol, val, tow, lg, vl = (torch.full((k,), 7.0, device="cuda:0") for k in (64, 1, 64 * 256, 64, 1))
+    net.debug_tower_dev(d_own, d_en, pol, val, tow, 0)
+    net.debug_heads_dev(d_own, d_en, pol, val, lg, vl, 0, tower_t=tow)
+    torch.cuda.synchronize()
+    assert all(bool((t == 7.0).all()) for t in (pol, val, tow, lg, vl))
 
 
 def test_tower_cluster_variants_vs_oracle_and_each_other():
