@@ -109,6 +109,21 @@ int rz_solve_deep(const uint64_t* own, const uint64_t* enemy, int8_t* move, int8
  * the same position could be misled by. */
 int rz_solve_deep_with_stop(const uint64_t* own, const uint64_t* enemy, int8_t* move, int8_t* score, size_t n, double timeout_s,
                             const volatile int32_t* stop, rz_deep_solve_stats* stats);
+/* The value of every legal move of one position (own to move), for endgame hints: bounds lo[sq] <= value <= hi[sq] of
+ * the move at sq, in the mover's frame (exact final disc difference, empties not awarded).  *legal receives the mover's
+ * legal mask, and lo / hi are meaningful on its squares only (0 elsewhere); with no legal move or more than 30 empties
+ * *legal = 0 and nothing is solved.  Every round is one forest with a root per open move at that move's own threshold
+ * (1, then 0, then the middle of its bounds), at most 8 rounds.  n_best >= 0 (0: every move): a move stops being refined
+ * once its hi is below the n_best-th largest lo.  On a normal return every move whose value is at least the n_best-th
+ * best value (ties included) has lo == hi, and every other move has hi below that value.  A timeout or the stop flag
+ * (nullable, as in rz_solve_deep_with_stop) ends the call within one slice plus the host's split time, with the bounds
+ * proven so far, which always hold.  on_round (nullable) is called on the calling thread after every round with the
+ * current bounds; it must not call back into the solver.  stats (nullable): `probes` counts the forests.  The rounds
+ * probe and fill the transposition table like rz_solve_deep's probes. */
+typedef void (*rz_deep_moves_cb)(const int8_t* lo, const int8_t* hi, void* user);
+int rz_solve_deep_moves(uint64_t own, uint64_t enemy, int n_best, double timeout_s, const volatile int32_t* stop,
+                        int8_t lo[64], int8_t hi[64], uint64_t* legal, rz_deep_moves_cb on_round, void* user,
+                        rz_deep_solve_stats* stats);
 /* Tuning of rz_solve_deep for tests and measurements: slice length (us), leaf target of the split and leaf floor
  * (empties below which the split stops); 0 restores each default (4000 us, one leaf per lane, 10 empties).  The next
  * call starts from an empty transposition table, so that it searches under the new tuning. */

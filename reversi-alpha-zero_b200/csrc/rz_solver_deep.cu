@@ -17,6 +17,9 @@
 //     machines look up the frames they enter and store the frames they decide, and resolve() stores the split-tree nodes
 //     it decides, which are the largest subtrees and the first ones the next probe revisits.
 // Booleans combine exactly, so the answer depends on nothing but the position (and on the timeout, only whether it hits).
+//
+// rz_solve_deep_moves asks the forest's other question, "every root decided": each round is one forest with one root per
+// root move still open, each at its own threshold, so every move's value is narrowed at once (solve_moves).
 #include <algorithm>
 #include <chrono>
 #include <vector>
@@ -36,17 +39,6 @@ constexpr int kDefaultSliceUs = 4000;
 constexpr int kDefaultLeafFloor = 10;
 constexpr int kCtxPerLane = 2;        // parked stacks per lane
 constexpr long long kDefaultTableBytes = 1LL << 30;
-
-enum : int32_t { kOpen = 0, kTrue = 1, kFalse = 2 };
-
-struct Node {  // 24 B, written by the host only
-    u64 own, enemy;
-    int32_t parent;  // -1: a root
-    int8_t t;        // the question: value(own to move) >= t ?
-    int8_t flip;     // 1: the node's answer is negated for its parent (opponent to move); 0: pass.  Roots: the wanted answer
-    int8_t empties;
-    int8_t leaf;
-};
 
 struct SliceArgs {
     const Node* nodes;
@@ -69,16 +61,6 @@ struct SliceArgs {
     Table table;
     unsigned long long* table_counts;  // kTabCounters
 };
-
-RZ_HD bool roots_answered(const volatile int32_t* status, const Node* nodes, int n_roots) {
-    // the lowest root whose answer is the wanted one, with every lower root decided the other way; or all decided
-    for (int i = 0; i < n_roots; ++i) {
-        const int s = status[i];
-        if (s == kOpen) return false;
-        if ((s == kTrue) == (nodes[i].flip != 0)) return true;
-    }
-    return true;
-}
 
 __device__ bool decided_above(const SliceArgs& a, int node) {
     const volatile int32_t* st = a.status;
@@ -277,9 +259,10 @@ struct Tree {
 
 struct ProbeRun {
     int slice_us, leaf_target, leaf_floor;
-    std::chrono::steady_clock::time_point deadline;
+    std::chrono::steady_clock::time_point t0, deadline;
     const volatile int32_t* stop;  // the caller's stop flag (nullable): nonzero ends the call like a timeout
     rz_deep_solve_stats* stats;
+    unsigned long long steps0;     // the workspace's node steps when the run began (with stats)
     bool expired() const { return (stop && *stop) || std::chrono::steady_clock::now() > deadline; }
 };
 
@@ -428,6 +411,30 @@ static int workspace(Workspace** out) {
     return RZ_OK;
 }
 
+// One solve's run under the current tuning, from now until `timeout_s` has passed or *stop is set; end_run fills the
+// node steps and seconds of its stats.
+static int begin_run(const Workspace& w, double timeout_s, const volatile int32_t* stop, rz_deep_solve_stats* stats, ProbeRun& P) {
+    P.t0 = std::chrono::steady_clock::now();
+    P.slice_us = g_tuning.slice_us ? g_tuning.slice_us : kDefaultSliceUs;
+    P.leaf_target = g_tuning.leaf_target ? g_tuning.leaf_target : w.lanes;
+    P.leaf_floor = g_tuning.leaf_floor ? g_tuning.leaf_floor : kDefaultLeafFloor;
+    P.deadline = P.t0 + std::chrono::duration_cast<std::chrono::steady_clock::duration>(std::chrono::duration<double>(timeout_s));
+    P.stop = stop;
+    P.stats = stats;
+    P.steps0 = 0;
+    if (stats) RZ_CUDA_TRY(cudaMemcpy(&P.steps0, w.total_steps, 8, cudaMemcpyDeviceToHost));
+    return RZ_OK;
+}
+
+static int end_run(const Workspace& w, const ProbeRun& P) {
+    if (!P.stats) return RZ_OK;
+    unsigned long long steps1 = 0;
+    RZ_CUDA_TRY(cudaMemcpy(&steps1, w.total_steps, 8, cudaMemcpyDeviceToHost));
+    P.stats->node_steps = (int64_t)(steps1 - P.steps0);
+    P.stats->seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - P.t0).count();
+    return RZ_OK;
+}
+
 // Bounds on the value of each root move, in the root mover's frame, learned from decided root children.
 struct MoveBounds {
     int lo[64], hi[64];
@@ -452,26 +459,30 @@ static void learn_root_children(const Tree& T, int root, MoveBounds& B, const in
     }
 }
 
+// The root moves of (own, enemy) in the split's order into child_sq; bounds [-64, 64], exact where the move ends the game.
+static int root_moves(u64 own, u64 enemy, u64 legal, int* child_sq, MoveBounds& B) {
+    int n_moves = 0;
+    for (int s = 0; s < 64; ++s) { B.lo[s] = -64; B.hi[s] = 64; }
+    const bool ordered = 64 - popc64(own | enemy) >= kOrderMinEmpties;
+    while (legal) {
+        const int a = solver::pick_move(own, enemy, legal, ordered);
+        legal &= ~(1ULL << a);
+        child_sq[n_moves++] = a;
+        LeafFrame c;
+        int diff;
+        if (!child_after(own, enemy, a, 0, c, diff)) B.lo[a] = B.hi[a] = diff;
+    }
+    return n_moves;
+}
+
 static int solve_one(Workspace& w, u64 own, u64 enemy, int8_t* move_out, int8_t* score_out, const ProbeRun& P) {
     *move_out = -1; *score_out = 0;
     const u64 legal = find_correct_moves(own, enemy);
     if (!legal || 64 - popc64(own | enemy) > kDeepMaxEmpties) return RZ_OK;
     // root moves in the split's order, and their exact values where the game ends
-    int child_sq[32], n_moves = 0;
+    int child_sq[kMaxRoots];
     MoveBounds B;
-    for (int s = 0; s < 64; ++s) { B.lo[s] = -64; B.hi[s] = 64; }
-    {
-        u64 m = legal;
-        const bool ordered = 64 - popc64(own | enemy) >= kOrderMinEmpties;
-        while (m) {
-            const int a = solver::pick_move(own, enemy, m, ordered);
-            m &= ~(1ULL << a);
-            child_sq[n_moves++] = a;
-            LeafFrame c;
-            int diff;
-            if (!child_after(own, enemy, a, 0, c, diff)) B.lo[a] = B.hi[a] = diff;
-        }
-    }
+    root_moves(own, enemy, legal, child_sq, B);
     Tree T;
     bool timed_out = false;
     auto probe = [&](int t, bool* r) -> int {
@@ -532,6 +543,59 @@ static int solve_one(Workspace& w, u64 own, u64 enemy, int8_t* move_out, int8_t*
     }
     if (best >= 64) return RZ_OK;  // cannot happen: some move reaches the value
     *move_out = (int8_t)best; *score_out = (int8_t)v;
+    return RZ_OK;
+}
+
+// Bounds B.lo <= value <= B.hi of every legal root move of (own, enemy), in the root mover's frame (rz_solve_deep_moves).
+// Each round is one forest with one root per open move, asking "does this move reach t?" at the move's own t (1, then
+// 0, then the middle of its bounds), and runs until every root is decided.  A move is open while it is inexact and, with
+// n_best > 0, its hi is not below the n_best-th largest lo.  lo / hi receive the bounds after every round, and on_round
+// (nullable) sees them.  On a timeout or stop the bounds proven so far stay, and they always hold.  The plan of each
+// round is plan_round (rz_solver_deep.cuh).
+static int solve_moves(Workspace& w, u64 own, u64 enemy, u64 legal, int n_best, int8_t* lo, int8_t* hi,
+                       rz_deep_moves_cb on_round, void* user, const ProbeRun& P) {
+    int child_sq[kMaxRoots];
+    MoveBounds B;
+    const int n_moves = root_moves(own, enemy, legal, child_sq, B);
+    auto publish = [&] {
+        for (int k = 0; k < n_moves; ++k) { lo[child_sq[k]] = (int8_t)B.lo[child_sq[k]]; hi[child_sq[k]] = (int8_t)B.hi[child_sq[k]]; }
+    };
+    publish();
+    Tree T;
+    for (int round = 0; round < kMaxMoveRounds; ++round) {
+        int lo_k[kMaxRoots], hi_k[kMaxRoots], t_k[kMaxRoots];
+        for (int k = 0; k < n_moves; ++k) { lo_k[k] = B.lo[child_sq[k]]; hi_k[k] = B.hi[child_sq[k]]; }
+        plan_round(lo_k, hi_k, n_moves, n_best, t_k);
+        int open_sq[kMaxRoots], t_of[kMaxRoots], n_open = 0;
+        bool pass_of[kMaxRoots];
+        T = Tree();
+        for (int k = 0; k < n_moves; ++k) {
+            if (t_k[k] == kNoProbe) continue;
+            const int s = child_sq[k], t = t_k[k];
+            LeafFrame c;
+            int diff;
+            child_after(own, enemy, s, t, c, diff);  // never a finished game: those are exact already
+            T.add(c.own, c.enemy, -1, c.t, kEveryRoot);
+            open_sq[n_open] = s; t_of[n_open] = t; pass_of[n_open++] = c.flip == 0;
+        }
+        if (!n_open) break;
+        T.n_roots = n_open;
+        if (P.stats) P.stats->probes += 1;
+        bool timed_out = false;
+        RZ_TRY(run_forest(w, T, P, &timed_out));
+        if (P.stats) P.stats->leaves += T.leaves;
+        // opponent to move: the move reaches t iff NOT (value_c >= 1 - t); pass: iff value_c >= t.  A root left open by a
+        // timeout proves nothing.
+        for (int k = 0; k < n_open; ++k) {
+            if (T.status[k] == kOpen) continue;
+            const int s = open_sq[k];
+            if ((T.status[k] == kTrue) == pass_of[k]) B.lo[s] = std::max(B.lo[s], t_of[k]);
+            else B.hi[s] = std::min(B.hi[s], t_of[k] - 1);
+        }
+        publish();
+        if (on_round) on_round(lo, hi, user);
+        if (timed_out) break;
+    }
     return RZ_OK;
 }
 
@@ -598,24 +662,28 @@ int rz_solve_deep_with_stop(const uint64_t* own, const uint64_t* enemy, int8_t* 
     for (size_t i = 0; i < n; ++i) {
         if (stats) stats[i] = rz_deep_solve_stats{};
         if (stop && *stop) { move[i] = -1; score[i] = 0; continue; }
-        const auto t0 = std::chrono::steady_clock::now();
         deep::ProbeRun P;
-        P.slice_us = deep::g_tuning.slice_us ? deep::g_tuning.slice_us : deep::kDefaultSliceUs;
-        P.leaf_target = deep::g_tuning.leaf_target ? deep::g_tuning.leaf_target : w->lanes;
-        P.leaf_floor = deep::g_tuning.leaf_floor ? deep::g_tuning.leaf_floor : deep::kDefaultLeafFloor;
-        P.deadline = t0 + std::chrono::duration_cast<std::chrono::steady_clock::duration>(std::chrono::duration<double>(timeout_s));
-        P.stop = stop;
-        P.stats = stats ? stats + i : nullptr;
-        unsigned long long steps0 = 0, steps1 = 0;
-        if (P.stats) RZ_CUDA_TRY(cudaMemcpy(&steps0, w->total_steps, 8, cudaMemcpyDeviceToHost));
+        RZ_TRY(deep::begin_run(*w, timeout_s, stop, stats ? stats + i : nullptr, P));
         RZ_TRY(deep::solve_one(*w, own[i], enemy[i], move + i, score + i, P));
-        if (P.stats) {
-            RZ_CUDA_TRY(cudaMemcpy(&steps1, w->total_steps, 8, cudaMemcpyDeviceToHost));
-            P.stats->node_steps = (int64_t)(steps1 - steps0);
-            P.stats->seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-        }
+        RZ_TRY(deep::end_run(*w, P));
     }
     return RZ_OK;
+}
+
+int rz_solve_deep_moves(uint64_t own, uint64_t enemy, int n_best, double timeout_s, const volatile int32_t* stop, int8_t* lo,
+                        int8_t* hi, uint64_t* legal, rz_deep_moves_cb on_round, void* user, rz_deep_solve_stats* stats) {
+    RZ_REQUIRE(lo && hi && legal, "rz_solve_deep_moves: null pointer");
+    RZ_REQUIRE(n_best >= 0, "rz_solve_deep_moves: negative n_best");
+    for (int s = 0; s < 64; ++s) lo[s] = hi[s] = 0;
+    if (stats) *stats = rz_deep_solve_stats{};
+    *legal = find_correct_moves(own, enemy);
+    if (!*legal || 64 - popc64(own | enemy) > deep::kDeepMaxEmpties) { *legal = 0; return RZ_OK; }
+    deep::Workspace* w = nullptr;
+    RZ_TRY(deep::workspace(&w));
+    deep::ProbeRun P;
+    RZ_TRY(deep::begin_run(*w, timeout_s, stop, stats, P));
+    RZ_TRY(deep::solve_moves(*w, own, enemy, *legal, n_best, lo, hi, on_round, user, P));
+    return deep::end_run(*w, P);
 }
 
 int rz_solve_deep(const uint64_t* own, const uint64_t* enemy, int8_t* move, int8_t* score, size_t n, double timeout_s,

@@ -38,6 +38,59 @@ struct LeafFrame {  // 32 B
 };
 static_assert(sizeof(LeafFrame) == 32, "leaf frame layout");
 
+// ------------------------------------------------------------------------------------------------------- probe forests
+//
+// A probe forest (rz_solver_deep.cu) is a node table whose roots are the probes' questions.  The kernel and the host's
+// copy of the tree ask roots_answered() whether the forest can end.
+
+enum : int32_t { kOpen = 0, kTrue = 1, kFalse = 2 };
+
+// `flip` of a root holds the forest's question: 0 or 1, the lowest root whose answer is that value (or all decided); or
+// kEveryRoot, every root decided.
+constexpr int kEveryRoot = 2;
+
+struct Node {  // 24 B, written by the host only
+    u64 own, enemy;
+    int32_t parent;  // -1: a root
+    int8_t t;        // the question: value(own to move) >= t ?
+    int8_t flip;     // 1: the node's answer is negated for its parent (opponent to move); 0: pass.  Roots: the question
+    int8_t empties;
+    int8_t leaf;
+};
+
+RZ_HD bool roots_answered(const volatile int32_t* status, const Node* nodes, int n_roots) {
+    // the lowest root whose answer is the wanted one, with every lower root decided the other way; or all decided
+    for (int i = 0; i < n_roots; ++i) {
+        const int s = status[i];
+        if (s == kOpen) return false;
+        const int f = nodes[i].flip;
+        if (f != kEveryRoot && (s == kTrue) == (f != 0)) return true;
+    }
+    return true;
+}
+
+// One round of rz_solve_deep_moves over n moves with bounds lo[k] <= value <= hi[k]: t[k] = the threshold its root asks
+// ("does the move reach t?": 1, then 0, then the middle of its bounds), or kNoProbe when the move is exact or, with
+// n_best > 0, its hi is below the n_best-th largest lo (it cannot be among the best n_best).  Returns the open moves.
+constexpr int kNoProbe = -128;
+constexpr int kMaxMoveRounds = 8;  // t = 1, t = 0 and six halvings narrow [-64, 64] to one value
+RZ_HD int plan_round(const int* lo, const int* hi, int n, int n_best, int* t) {
+    int cut = -65;
+    if (n_best > 0 && n_best <= n)
+        for (int k = 0; k < n; ++k) {  // the n_best-th largest lo: the largest lo with n_best values at least as large
+            int at_least = 0;
+            for (int j = 0; j < n; ++j) at_least += lo[j] >= lo[k];
+            if (at_least >= n_best && lo[k] > cut) cut = lo[k];
+        }
+    int open = 0;
+    for (int k = 0; k < n; ++k) {
+        const int l = lo[k], h = hi[k];
+        t[k] = l >= h || h < cut ? kNoProbe : l <= 0 && h >= 1 ? 1 : l <= -1 && h >= 0 ? 0 : l + (h - l + 1) / 2;
+        open += t[k] != kNoProbe;
+    }
+    return open;
+}
+
 // ------------------------------------------------------------------------------------------------ transposition table
 //
 // An HBM array of buckets of kTableWays entries (one 128-byte line), indexed by the lane solver's position hash.  An

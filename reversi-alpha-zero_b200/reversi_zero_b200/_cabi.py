@@ -63,6 +63,10 @@ class DeepSolveStats(C.Structure):
                 ("leaves", C.c_int64), ("node_steps", C.c_int64), ("seconds", C.c_double)]
 
 
+# rz_deep_moves_cb: (lo int8[64], hi int8[64], user)
+DeepMovesCallback = C.CFUNCTYPE(None, i8p, i8p, vp)
+
+
 class DeepTableStats(C.Structure):
     _fields_ = [(n, C.c_int64) for n in ("lookups", "cutoffs", "hints", "stores", "replaced", "merges", "dropped",
                                          "occupied", "bytes")]
@@ -92,6 +96,8 @@ SIGNATURES = {
     "rz_solve": (C.c_int, [u64p, u64p, u8p, i8p, i8p, sz]),
     "rz_solve_deep": (C.c_int, [u64p, u64p, i8p, i8p, sz, C.c_double, C.POINTER(DeepSolveStats)]),
     "rz_solve_deep_with_stop": (C.c_int, [u64p, u64p, i8p, i8p, sz, C.c_double, C.POINTER(C.c_int32), C.POINTER(DeepSolveStats)]),
+    "rz_solve_deep_moves": (C.c_int, [C.c_uint64, C.c_uint64, C.c_int, C.c_double, C.POINTER(C.c_int32), i8p, i8p, u64p,
+                                      DeepMovesCallback, vp, C.POINTER(DeepSolveStats)]),
     "rz_solve_deep_tune": (C.c_int, [C.c_int, C.c_int, C.c_int]),
     "rz_solve_deep_table": (C.c_int, [C.c_int64]),
     "rz_solve_deep_clear": (C.c_int, []),

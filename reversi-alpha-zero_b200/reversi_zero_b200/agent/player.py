@@ -32,6 +32,15 @@ def solver_max_empties(config):
     return int(getattr(getattr(config, "b200", None), "solver_max_empties", 12))
 
 
+def solves_exactly(play_config, own, enemy, max_empties=64):
+    """True where ReversiPlayer asks its exact root solver: ``use_solver_turn`` set and the turn (discs - 4) at least
+    that.  With `max_empties`, also at most that many empty squares: the positions the solver answers rather than
+    refuses, which the game analysis and NBoard's exact hints solve."""
+    use_solver_turn = getattr(play_config, "use_solver_turn", None)
+    discs = bit_count(own) + bit_count(enemy)
+    return bool(use_solver_turn) and discs - 4 >= use_solver_turn and 64 - discs <= max_empties
+
+
 def search_play_config(config, play_config):
     """The search parameters ReversiPlayer's engine runs with: `play_config`, except that the reference reads three of
     them from config.play even when a separate play_config is given (evaluate.py / play_game callers):
@@ -72,8 +81,8 @@ class ReversiPlayer:
         return MCTSInfo(defaultdict(lambda: np.zeros((64,))), defaultdict(lambda: np.zeros((64,))),
                         defaultdict(lambda: np.zeros((64,))))
 
-    def action(self, own, enemy, callback_in_mtcs=None):
-        return self.action_with_evaluation(own, enemy, callback_in_mtcs=callback_in_mtcs).action
+    def action(self, own, enemy, callback_in_mtcs=None, solve=True):
+        return self.action_with_evaluation(own, enemy, callback_in_mtcs=callback_in_mtcs, solve=solve).action
 
     def _search(self, own, enemy):
         """simulation_num_per_move simulations from (own, enemy); with a CallbackInMCTS the search runs in chunks of
@@ -96,14 +105,15 @@ class ReversiPlayer:
                 cb.callback(list(w / (n + 1e-5)), list(n))
         return n.astype(np.float64), w.astype(np.float64)
 
-    def action_with_evaluation(self, own, enemy, callback_in_mtcs=None):
+    def action_with_evaluation(self, own, enemy, callback_in_mtcs=None, solve=True):
         """agent/player.py:82-134; the exact root solver (:100-103,150-161) runs through lib/reversi_solver (rz_solve), the
-        WLD solver inside simulations (:237-251) inside the engine."""
+        WLD solver inside simulations (:237-251) inside the engine.  solve=False searches even where the root solver would
+        answer (NBoard's hint, after an exact solve that proved nothing)."""
         pc = self.play_config
         turn = bit_count(own) + bit_count(enemy) - 4
         self.callback_in_mtcs = callback_in_mtcs
         self.requested_stop_thinking = False
-        if pc.use_solver_turn and turn >= pc.use_solver_turn:  # action_by_searching, agent/player.py:100-103,150-161
+        if solve and solves_exactly(pc, own, enemy):  # action_by_searching, agent/player.py:100-103,150-161
             if self.solver is None:
                 from ..lib import reversi_solver
                 self.solver = reversi_solver.ReversiSolver(solver_max_empties(self.config))

@@ -134,6 +134,7 @@ class B200Config(_Section):
         self.train_devices = None   # opt: CUDA ordinals of a data-parallel training group, e.g. [0, 1]; None = the one device
         self.solver_max_empties = 12  # ReversiPlayer's exact root solver: 13..this many empties go to the whole-GPU solver
         self.nboard_analyze = False  # NBoard: answer `analyze` with a retrograde analysis of the game (play_game/analysis.py)
+        self.nboard_exact_hint = False  # NBoard: in solver range, `hint n` reports every move's exact value (100% lines)
         self.keep_promoted_models = False  # eval: archive every promoted blob under <model_dir>/promoted/ (worker/evaluate.py)
 
 

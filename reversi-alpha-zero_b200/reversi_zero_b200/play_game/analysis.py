@@ -22,7 +22,7 @@ from logging import getLogger
 
 import numpy as np
 
-from ..agent.player import search_play_config, solver_max_empties
+from ..agent.player import search_play_config, solver_max_empties, solves_exactly
 from ..engine import Engine, engine_cfg_from_play_config, EVAL_NET, EVAL_FAKE
 from ..lib.bitboard import find_correct_moves, calc_flip, bit_count
 
@@ -82,12 +82,10 @@ def analyse(positions, play_config, max_empties, report, stopped, solve_lane, so
       search(own list, enemy list) -> list of values (10 * q), or None when stopped.
     Returns False when stopped, else True."""
     kinds = classify(positions)
-    use_solver_turn = getattr(play_config, "use_solver_turn", None)
     value = {}   # (own, enemy) -> (value for its mover, exact)
 
     def solvable(own, enemy):
-        discs = bit_count(own) + bit_count(enemy)
-        return bool(use_solver_turn) and discs - 4 >= use_solver_turn and 64 - discs <= max_empties
+        return solves_exactly(play_config, own, enemy, max_empties)
 
     targets = []   # (own, enemy) to evaluate, without repeats, in game order
     for kind, _, own, enemy in kinds:

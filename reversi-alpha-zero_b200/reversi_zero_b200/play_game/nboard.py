@@ -7,15 +7,18 @@ Commands arrive on stdin, one per line; stdout carries protocol replies only (lo
 the device; the tree is kept across the moves of a game and dropped when NBoard sends the opening position.  A
 ``ping`` interrupts a running search from the reader thread, so NBoard gets its ``pong`` as soon as the current chunk
 of ``hint_callback_per_sim`` simulations ends.  With ``b200.nboard_analyze`` on, ``analyze`` answers with a retrograde
-analysis of the game (play_game/analysis.py), which a ``ping`` interrupts as well.
+analysis of the game (play_game/analysis.py), which a ``ping`` interrupts as well.  With ``b200.nboard_exact_hint`` on,
+``hint n`` in a position the player would solve reports the exact value of the best n moves (``100%`` lines, after
+``100%W`` lines for moves whose sign is proven first); a ``ping`` interrupts it within one slice of the deep solver.
 """
+import ctypes as C
 import re
 import sys
 from collections import namedtuple
 from logging import getLogger, StreamHandler, FileHandler
 from time import time
 
-from ..agent.player import ReversiPlayer, CallbackInMCTS
+from ..agent.player import ReversiPlayer, CallbackInMCTS, solver_max_empties, solves_exactly
 from ..env.reversi_env import ReversiEnv, Player
 from ..lib.ggf import parse_ggf, convert_to_bitboard_and_actions, convert_move_to_action, convert_action_to_move
 from ..lib.nonblocking_stream_reader import NonBlockingStreamReader
@@ -26,6 +29,8 @@ logger = getLogger(__name__)
 GameState = namedtuple("GameState", "black white actions player")
 GoResponse = namedtuple("GoResponse", "action eval time")
 HintResponse = namedtuple("HintResponse", "action value visit")
+ExactHint = namedtuple("ExactHint", "action value depth")   # depth: "100%" exact, "100%W" win/loss proven
+HINT_TIMEOUT = 30   # the reference solver's timeout (ReversiSolver.solve)
 
 
 def start(config):
@@ -43,6 +48,10 @@ class NBoardEngine:
     # play_game.analysis.GameAnalyser, created at the first analysis.  A class attribute, so that the reader thread's
     # push_callback finds it on every engine, also one whose analysis has never run.
     analyser = None
+    # the exact hint's solver and its stop flag (a ctypes.c_int32), created at the first exact hint; class attributes for
+    # the same reason
+    hint_solver = None
+    hint_stop = None
 
     def __init__(self, config, stdin=None, stdout=None):
         self.config = config
@@ -85,6 +94,8 @@ class NBoardEngine:
             self.stop_thinking()
             if self.analyser is not None:
                 self.analyser.stop()
+            if self.hint_stop is not None:
+                self.hint_stop.value = 1
 
     def stop(self):
         self.running = False
@@ -149,6 +160,10 @@ class NBoardEngine:
 
     def hint(self, n_hint):
         states = self._states()
+        exact = getattr(getattr(self.config, "b200", None), "nboard_exact_hint", False) and \
+            solves_exactly(self.play_config, *states, solver_max_empties(self.config))
+        if exact and self.exact_hint(*states, n_hint):
+            return
 
         def hint_report_callback(values, visits):
             hint_list = []
@@ -157,9 +172,35 @@ class NBoardEngine:
                     hint_list.append(HintResponse(action, values[action], visit))
             self.handler.report_hint(hint_list)
 
-        self.player.action(*states, callback_in_mtcs=CallbackInMCTS(self.nc.hint_callback_per_sim, hint_report_callback))
+        # after an exact solve that proved nothing (a timeout), the search answers without solving again
+        self.player.action(*states, callback_in_mtcs=CallbackInMCTS(self.nc.hint_callback_per_sim, hint_report_callback),
+                           solve=not exact)
         item = self.player.ask_thought_about(*states)
         hint_report_callback(item.values, item.visit)
+
+    def exact_hint(self, own, enemy, n_hint):
+        """`hint n` with b200.nboard_exact_hint on, in solver range: the value of every move from the exact solvers
+        (ReversiSolver.solve_moves, n_best = n, the solver's 30 s timeout), reported as it is proven: after each deep round
+        a `100%W` line for every move whose sign is proven before its value, then the best n proven moves.  A ping stops
+        the solve and nothing more is sent.  False when nothing was proven, not even a sign: then the search answers."""
+        if self.hint_solver is None:
+            from ..lib.reversi_solver import ReversiSolver
+            self.hint_solver = ReversiSolver(solver_max_empties(self.config))
+            self.hint_stop = C.c_int32(0)
+        self.hint_stop.value = 0
+
+        def on_bounds(bounds):
+            if not self.hint_stop.value:
+                self.handler.report_exact_hint(wld_hints(bounds))
+
+        bounds = self.hint_solver.solve_moves(own, enemy, 1, n_hint, HINT_TIMEOUT, self.hint_stop, on_bounds)
+        if self.hint_stop.value:
+            return True
+        hints = exact_hints(bounds or {}, n_hint)
+        if not hints:
+            return False
+        self.handler.report_exact_hint(hints)
+        return True
 
 
     def begin_analysis(self):
@@ -175,6 +216,28 @@ class NBoardEngine:
             return
         black, white, player = self.game_start
         self.analyser.analyse(black, white, player, self.game_actions, report)
+
+
+def _best_last(hints):
+    """ascending value, and among equal values the lowest square last: NBoard takes the last line as the best, and it
+    is then go's move"""
+    return sorted(hints, key=lambda h: (h.value, -h.action))
+
+
+def wld_hints(bounds):
+    """The `100%W` hints of a deep round's bounds {square: (lo, hi)}: every move whose sign is proven and whose value
+    is not, with lo for a proven win and hi for a proven loss"""
+    out = [ExactHint(s, lo if lo >= 1 else hi, "100%W") for s, (lo, hi) in bounds.items()
+           if lo < hi and (lo >= 1 or hi <= -1)]
+    return _best_last(out)
+
+
+def exact_hints(bounds, n_hint):
+    """The final hint list of a solve: the best `n_hint` (0: all) of the moves with an exact value (`100%`) or a proven
+    sign (`100%W`, as in wld_hints; only after a timeout), best last"""
+    out = [ExactHint(s, lo, "100%") for s, (lo, hi) in bounds.items() if lo == hi] + wld_hints(bounds)
+    out.sort(key=lambda h: (-h.value, h.action))
+    return _best_last(out[:n_hint] if n_hint > 0 else out)
 
 
 def analysis_line(moves_made, value, exact):
@@ -241,6 +304,12 @@ class NBoardProtocolVersion2:
         for hint in reversed(hint_list):  # NBoard takes the last line as the best
             move = convert_action_to_move(hint.action)
             self.engine.reply(f"search {move} {hint.value} 0 {int(hint.visit)}")
+
+    def report_exact_hint(self, hints):
+        """ExactHint lines, already in NBoard's order (best last): `search {move} {disc difference} 0 100%` for an
+        exact value, `... 100%W` for a proven win (lower bound) or loss (upper bound)"""
+        for hint in hints:
+            self.engine.reply(f"search {convert_action_to_move(hint.action)} {int(hint.value)} 0 {hint.depth}")
 
     def go(self):
         """Replies "=== {move}/{eval}/{time}"; the engine's board is not changed (NBoard sends a "move" next)."""
