@@ -148,6 +148,18 @@ int rz_solve_deep_table(int64_t bytes);
 int rz_solve_deep_clear(void);
 int rz_solve_deep_table_stats(rz_deep_table_stats* out);
 
+/* Every distinct opening of `plies` plies (1..12), enumerated on the current device (csrc/rz_openings.cu).  Two move
+ * sequences are the same opening when they reach the same position up to the 8 board symmetries (transpositions
+ * included); a sequence through a position whose side to move must pass, or whose game is over, is not an opening.  Each
+ * opening is represented by the sequence that is least by (parent opening, move square) at every ply, in the orientation
+ * that sequence reaches.  Output, host buffers, in ascending order of the canonical key (the least (own, enemy) pair over
+ * the 8 images, own compared first): own[i] / enemy[i] = the position reached, in the mover's frame; moves[i * plies + j]
+ * = its j-th move (square 0..63).  cap = 0: only *n_out is set (the outputs may be NULL); cap < *n_out: RZ_ECAPACITY.
+ * level_counts (nullable, plies + 1 entries): the number of openings of 0 .. plies plies.  Repeated calls give identical
+ * output.  Device memory grows with the level; a level that does not fit returns RZ_ENOMEM.  Synchronous. */
+int rz_openings_enumerate(int plies, uint64_t* own, uint64_t* enemy, uint8_t* moves, size_t cap, size_t* n_out,
+                          uint64_t* level_counts);
+
 /* Scalar host twins for the single-environment Python objects (ReversiEnv / Board used by the
  * reference's evaluate.py, nboard.py, game_model.py): same header-only code as the device kernels
  * (csrc/rz_bitboard.cuh), compiled for the host.  Not a fallback for the batched path. */
@@ -322,7 +334,7 @@ typedef struct rz_game {
     uint8_t turn;           /* ReversiEnv.turn at the end */
     uint8_t black_net;      /* matches and leagues: index of the network that played black (0 in self-play) */
     uint8_t white_net;      /* ... and white (0 in self-play, 1 - black_net in a two-network match) */
-    uint8_t pad;
+    uint8_t opening_plies;  /* plies of the opening the game started from (rz_engine_set_openings; 0 without one) */
     int32_t table_nodes;    /* positions in the slot's statistics table at the end of the game (half of the reference's
                                len(mtcs_info.var_p), which also holds every colour-swapped mirror key, worker/self_play.py:127) */
     int32_t pad2;
@@ -395,6 +407,17 @@ int rz_engine_set_nets(rz_engine* e, rz_net* const* nets, const float* fake_scal
                        const uint8_t* white_net, uint64_t n_games);
 /* update the resignation rule for decisions taken from now on (SelfPlayWorker's threshold auto-tuner,
  * worker/self_play.py:250-260). */
+/* games from openings: the game with local index i (< n_games) starts after the n_moves[i] squares at
+ * moves[i * RZ_MAX_OPENING_PLIES ...], which the engine plays without a search and does not record; n_moves[i] = 0 is the
+ * initial position (a table of zeros gives the games of no table).  The game's turn and side to move then follow from the
+ * opening (change_tau_turn, allowed_resign_turn and use_solver_turn count from the initial position), a game with an
+ * opening has no forced first move, its statistics start empty at the opening's position, and rz_game.opening_plies
+ * reports the length.  Works with one network, rz_engine_set_second_net and rz_engine_set_nets.  RZ_EINVAL, with the engine
+ * unchanged: an illegal move, a move after which the other side must pass, a move that ends the game, more than
+ * RZ_MAX_OPENING_PLIES moves, max_games 0 or greater than n_games (rz_engine_set_max_games then keeps to that bound),
+ * warm_start on, or a call after the first wave. */
+#define RZ_MAX_OPENING_PLIES 20
+int rz_engine_set_openings(rz_engine* e, const uint8_t* moves, const uint8_t* n_moves, uint64_t n_games);
 int rz_engine_set_resign_threshold(rz_engine* e, int use_resign_threshold, float resign_threshold);
 /* single-position search (ReversiPlayer.action outside the self-play loop: evaluate.py, nboard.py, GUI; also the
  * parity-test hook): every slot searches (own, enemy) with `player` to move for simulation_num_per_move

@@ -120,10 +120,12 @@ struct Slot {
     u64 root_own, root_enemy;
     uint8_t root_pid, black_net, white_net;  // black_net / white_net: networks of the two colours (matches, leagues)
     uint8_t root_req;         // 1: an exact root solve has to be put into this wave's solver batch
+    uint8_t opening_plies;    // plies of the game's opening (rz_engine_set_openings), replayed before its first search
     uint32_t ply_waves;       // waves this slot has spent on the ply being decided (rz_ply::waves)
     uint32_t n_solves, n_searched_plies;
 };
 
+constexpr int kOpeningStride = RZ_MAX_OPENING_PLIES + 1;
 constexpr int kCacheTurnBuckets = 61;  // turns 0..59 of the searched root; 60: the warm-started first game of a slot
 
 struct Status {
@@ -169,6 +171,7 @@ struct DevPtrs {
     float* policy;         // [net][G*K][64]
     float* value;          // [net][G*K]
     const uint8_t* net_table;  // [game][2]: networks of black and white (rz_engine_set_nets); NULL: alternate with the game
+    const uint8_t* openings;   // [game][kOpeningStride]: number of plies, then the squares (rz_engine_set_openings); NULL: none
     // endgame solver: one resumable request context per descent (+ one per slot for the exact root solve), the lists of
     // unfinished requests (per group, double-buffered by wave parity) and the network results a waiting slot has to keep
     solver::SolveCtx* sctx;  // [G][K + 1]
@@ -270,6 +273,8 @@ struct rz_engine {
     int row_nets;                   // networks the row buffers and batch counters have room for
     uint8_t* d_net_table;           // rz_engine_set_nets: [game][2] on the device (NULL: none)
     uint64_t net_table_games;
+    uint8_t* d_openings;            // rz_engine_set_openings: [game][kOpeningStride] on the device (NULL: none)
+    uint64_t opening_games;
     int device;
     cudaStream_t stream;      // group 0 + all host<->device traffic
     cudaStream_t stream2;     // group 1 (tick of one group overlaps the network launch of the other)
@@ -526,6 +531,7 @@ int rz_engine_create(const rz_engine_cfg* cfg, rz_net* net, int device, rz_engin
     e->nets[0] = net;
     e->row_nets = 2;
     e->d_net_table = nullptr; e->net_table_games = 0;
+    e->d_openings = nullptr; e->opening_games = 0;
     e->waves = e->nn_launches = e->mcts_launches = e->finished_total = 0;
     e->h_status = nullptr; e->h_flags = nullptr; e->stream = nullptr; e->stream2 = nullptr;
     e->ev_used = 0; e->nn_ms = e->mcts_ms = e->run_ms = 0.0;
@@ -581,6 +587,7 @@ int rz_engine_create(const rz_engine_cfg* cfg, rz_net* net, int device, rz_engin
     if (!rc) rc = dev_alloc(e, (void**)&p.mail_flag, G * 2, true);
     if (!rc) rc = dev_alloc(e, (void**)&p.status, sizeof(Status), true);
     p.net_table = nullptr;
+    p.openings = nullptr;
     if (!rc) rc = dev_alloc(e, (void**)&p.batch_count, (size_t)e->row_nets * 2 * 64 * sizeof(uint32_t), true);
     if (!rc) rc = dev_alloc(e, (void**)&p.batch_own, (B + 2) * sizeof(u64), true);
     if (!rc) rc = dev_alloc(e, (void**)&p.batch_enemy, (B + 2) * sizeof(u64), true);
@@ -751,6 +758,9 @@ int rz_engine_set_max_games(rz_engine* e, uint64_t max_games) {
     RZ_REQUIRE(!e->dp.net_table || (max_games >= 1 && max_games <= e->net_table_games),
                "rz_engine_set_max_games: %llu games with a network table of %llu games", (unsigned long long)max_games,
                (unsigned long long)e->net_table_games);
+    RZ_REQUIRE(!e->dp.openings || (max_games >= 1 && max_games <= e->opening_games),
+               "rz_engine_set_max_games: %llu games with an opening table of %llu games", (unsigned long long)max_games,
+               (unsigned long long)e->opening_games);
     e->dc.max_games = max_games;
     e->cfg.max_games = max_games;
     return RZ_OK;
@@ -817,6 +827,54 @@ int rz_engine_set_nets(rz_engine* e, rz_net* const* nets, const float* fake_scal
     RZ_TRY(arena_swap(e, (void**)&e->d_net_table, d_table));
     e->net_table_games = n_games;
     use_nets(e, nets, fake_scale, n_nets, e->d_net_table);
+    return RZ_OK;
+}
+
+int rz_engine_set_openings(rz_engine* e, const uint8_t* moves, const uint8_t* n_moves, uint64_t n_games) {
+    RZ_REQUIRE(e && moves && n_moves, "rz_engine_set_openings: null pointer");
+    RZ_REQUIRE(e->waves == 0, "rz_engine_set_openings: must be called before the first wave");
+    RZ_REQUIRE(!e->dc.warm_start, "rz_engine_set_openings: warm_start already chooses where the first games begin");
+    RZ_REQUIRE(e->dc.max_games >= 1 && e->dc.max_games <= n_games,
+               "rz_engine_set_openings: max_games = %llu must be 1..n_games (%llu): the table has no entry for later games",
+               (unsigned long long)e->dc.max_games, (unsigned long long)n_games);
+    std::vector<uint8_t> table((size_t)n_games * kOpeningStride, 0);
+    for (uint64_t i = 0; i < n_games; ++i) {
+        const int n = n_moves[i];
+        RZ_REQUIRE(n <= RZ_MAX_OPENING_PLIES, "rz_engine_set_openings: game %llu: %d moves, at most %d", (unsigned long long)i, n,
+                   RZ_MAX_OPENING_PLIES);
+        // the env would end a game at an illegal move; an opening must be legal, and never pass or finish the game
+        EnvState env;
+        env_reset(env);
+        for (int j = 0; j < n; ++j) {
+            const int mv = moves[i * RZ_MAX_OPENING_PLIES + j];
+            const bool b = env.next_player == 1;
+            const u64 legal = mv < 64 ? find_correct_moves(b ? env.black : env.white, b ? env.white : env.black) : 0;
+            RZ_REQUIRE((legal >> mv) & 1, "rz_engine_set_openings: game %llu: move %d (square %d) is illegal", (unsigned long long)i, j + 1, mv);
+            const uint8_t mover = env.next_player;
+            env_step(env, mv);
+            RZ_REQUIRE(!env.done, "rz_engine_set_openings: game %llu: move %d ends the game", (unsigned long long)i, j + 1);
+            RZ_REQUIRE(env.next_player != mover, "rz_engine_set_openings: game %llu: after move %d the other side must pass",
+                       (unsigned long long)i, j + 1);
+            table[(size_t)i * kOpeningStride + 1 + j] = (uint8_t)mv;
+        }
+        table[(size_t)i * kOpeningStride] = (uint8_t)n;
+    }
+    RZ_CUDA_TRY(cudaSetDevice(e->device));
+    uint8_t* d_table = nullptr;
+    if (cudaMalloc((void**)&d_table, table.size()) != cudaSuccess) {
+        cudaGetLastError();
+        set_error("rz_engine_set_openings: cudaMalloc(%zu bytes) failed", table.size());
+        return RZ_ENOMEM;
+    }
+    const cudaError_t ce = cudaMemcpy(d_table, table.data(), table.size(), cudaMemcpyHostToDevice);
+    if (ce != cudaSuccess) {
+        cudaFree(d_table);
+        set_error("rz_engine_set_openings: cudaMemcpy: %s", cudaGetErrorString(ce));
+        return RZ_ECUDA;
+    }
+    RZ_TRY(arena_swap(e, (void**)&e->d_openings, d_table));
+    e->opening_games = n_games;
+    e->dp.openings = e->d_openings;
     return RZ_OK;
 }
 

@@ -429,6 +429,19 @@ struct WCtx {
         begin_ply(b2 ? sl.env.black : sl.env.white, b2 ? sl.env.white : sl.env.black, sl.env.next_player);
     }
 
+    // rz_engine_set_openings (max_games bounds `local` by the table's length): the opening's plies are played without a
+    // search and not recorded; the host checked that none passes or ends the game.  Kept out of line: inlined into the
+    // tick kernel it costs new_game's callers registers.
+    __device__ __noinline__ void play_opening(u64 local) {
+        const uint8_t* op = p.openings + local * kOpeningStride;
+        sl.opening_plies = op[0];
+        for (int i = 0; i < (int)sl.opening_plies; ++i) env_step(sl.env, op[1 + i]);
+        if (sl.opening_plies) {
+            const bool b = sl.env.next_player == 1;
+            begin_ply(b ? sl.env.black : sl.env.white, b ? sl.env.white : sl.env.black, sl.env.next_player);
+        }
+    }
+
     __device__ void new_game() {
         const u64 local = (u64)s + sl.games_played * (u64)c.G;
         if (c.max_games && local >= c.max_games) {
@@ -467,6 +480,8 @@ struct WCtx {
         sl.enable_resign = (uint8_t)((double)c.disable_resignation_rate <= u01(draw(c.seed, sl.game_id, 0, P_GAME, 0).x));
         if (lane == 0) atomicAdd(&p.status->games_started, 1ULL);
         sl.phase = PH_DECIDE;
+        sl.opening_plies = 0;
+        if (p.openings) play_opening(local);
         if (c.warm_start && sl.games_played == 1) {
             // the slot's first game starts at turn `pre` (drawn from the profile, rz_engine_set_warm_start_profile) after
             // `pre` random legal plies, and its first search is a uniformly drawn part of a whole one: the state of a slot
@@ -514,7 +529,7 @@ struct WCtx {
             g.first_ply = 0; g.n_plies = (int32_t)sl.ply; g.expansions = (int32_t)sl.n_expand; g.simulations = (int32_t)sl.n_sims;
             g.winner = sl.env.winner; g.black_z = sl.env.winner == 1 ? 1 : (sl.env.winner == 2 ? -1 : 0);
             g.resign_enabled = sl.enable_resign; g.resigned_mask = sl.resigned_mask; g.turn = sl.env.turn;
-            g.black_net = sl.black_net; g.white_net = sl.white_net; g.pad = 0;
+            g.black_net = sl.black_net; g.white_net = sl.white_net; g.opening_plies = sl.opening_plies;
             g.table_nodes = (int32_t)sl.n_nodes; g.pad2 = 0;
             atomicMax(&p.status->max_nodes, (unsigned long long)sl.n_nodes);
             atomicMax(&p.status->max_edges, (unsigned long long)sl.n_edges);

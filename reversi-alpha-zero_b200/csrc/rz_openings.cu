@@ -1,0 +1,211 @@
+// rz_openings.cu -- every distinct opening of p plies, enumerated on the device (rz_openings_enumerate).
+//
+// Level by level from the initial position: each frontier position is expanded to its children (rz_openings.cuh), the
+// children are sorted by their canonical key (two stable CUB radix sorts, low word then high word, so that equal keys
+// stay in child order), and the first child of every key -- the one with the least (parent index, move square) -- becomes
+// the class's representative, in the orientation its own moves reach.  The representatives, in ascending key order, are
+// the next frontier.  Every step is a scan, a stable sort or a gather: the output does not depend on the schedule.
+#include <climits>
+#include <cub/cub.cuh>
+#include <vector>
+
+#include "rz_common.cuh"
+#include "rz_openings.cuh"
+
+namespace rz {
+namespace openings {
+
+constexpr int kThreads = 256;
+
+inline unsigned blocks_for(size_t n) { return (unsigned)((n + kThreads - 1) / kThreads); }
+
+__global__ void __launch_bounds__(kThreads) count_kernel(const u64* __restrict__ own, const u64* __restrict__ enemy, size_t n,
+                                                         uint64_t* __restrict__ count) {
+    const size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x;
+    if (i < n) count[i] = (uint64_t)popc64(kept_moves(own[i], enemy[i]));
+}
+
+// children of parent i at offset[i] .. : canonical key, the child's index (the sort's value) and parent * 64 + square
+__global__ void __launch_bounds__(kThreads) expand_kernel(const u64* __restrict__ own, const u64* __restrict__ enemy, size_t n,
+                                                          const uint64_t* __restrict__ offset, u64* __restrict__ k_hi,
+                                                          u64* __restrict__ k_lo, uint32_t* __restrict__ index,
+                                                          u64* __restrict__ origin) {
+    const size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x;
+    if (i >= n) return;
+    const u64 o = own[i], e = enemy[i];
+    size_t c = offset[i];
+    for (u64 m = find_correct_moves(o, e); m; m &= m - 1) {
+        const int sq = ctz64(m);
+        u64 co, ce;
+        if (!child(o, e, sq, co, ce)) continue;
+        canonical(co, ce, k_hi[c], k_lo[c]);
+        index[c] = (uint32_t)c;
+        origin[c] = (u64)i * 64 + (u64)sq;
+        ++c;
+    }
+}
+
+__global__ void __launch_bounds__(kThreads) gather_kernel(const u64* __restrict__ src, const uint32_t* __restrict__ index, size_t n,
+                                                          u64* __restrict__ dst) {
+    const size_t j = (size_t)blockIdx.x * kThreads + threadIdx.x;
+    if (j < n) dst[j] = src[index[j]];
+}
+
+// head[j] = 1 where the sorted key j differs from key j - 1 (k_hi sorted, k_lo in child order)
+__global__ void __launch_bounds__(kThreads) head_kernel(const u64* __restrict__ hi_sorted, const u64* __restrict__ k_lo,
+                                                        const uint32_t* __restrict__ index, size_t n, uint8_t* __restrict__ head) {
+    const size_t j = (size_t)blockIdx.x * kThreads + threadIdx.x;
+    if (j >= n) return;
+    head[j] = j == 0 || hi_sorted[j] != hi_sorted[j - 1] || k_lo[index[j]] != k_lo[index[j - 1]];
+}
+
+// next frontier: representative k is child rep[k]; its position and moves (its parent's moves, then its square)
+__global__ void __launch_bounds__(kThreads) next_kernel(const u64* __restrict__ own, const u64* __restrict__ enemy,
+                                                        const uint8_t* __restrict__ moves, int level, int stride,
+                                                        const uint32_t* __restrict__ rep, const u64* __restrict__ origin, size_t n,
+                                                        u64* __restrict__ own_out, u64* __restrict__ enemy_out,
+                                                        uint8_t* __restrict__ moves_out) {
+    const size_t k = (size_t)blockIdx.x * kThreads + threadIdx.x;
+    if (k >= n) return;
+    const u64 org = origin[rep[k]];
+    const size_t parent = (size_t)(org >> 6);
+    const int sq = (int)(org & 63);
+    u64 co, ce;
+    child(own[parent], enemy[parent], sq, co, ce);
+    own_out[k] = co;
+    enemy_out[k] = ce;
+    for (int j = 0; j < level; ++j) moves_out[k * stride + j] = moves[parent * stride + j];
+    moves_out[k * stride + level] = (uint8_t)sq;
+}
+
+// device buffers of one call, freed on every return
+struct Buffers {
+    std::vector<void*> held;
+    ~Buffers() { for (void* p : held) cudaFree(p); }
+    template <typename T>
+    int get(T** out, size_t count) {
+        void* p = nullptr;
+        const size_t bytes = count ? count * sizeof(T) : 1;
+        if (cudaMalloc(&p, bytes) != cudaSuccess) {
+            cudaGetLastError();
+            set_error("rz_openings_enumerate: cudaMalloc(%zu bytes) failed", bytes);
+            return RZ_ENOMEM;
+        }
+        held.push_back(p);
+        *out = (T*)p;
+        return RZ_OK;
+    }
+    void release(void* p) {
+        for (size_t i = 0; i < held.size(); ++i)
+            if (held[i] == p) { cudaFree(p); held.erase(held.begin() + (long)i); return; }
+    }
+};
+
+}  // namespace openings
+}  // namespace rz
+
+using namespace rz;
+using namespace rz::openings;
+
+extern "C" int rz_openings_enumerate(int plies, uint64_t* own_out, uint64_t* enemy_out, uint8_t* moves_out, size_t cap,
+                                     size_t* n_out, uint64_t* level_counts) {
+    RZ_REQUIRE(plies >= 1 && plies <= 12, "rz_openings_enumerate: plies = %d outside 1..12", plies);
+    RZ_REQUIRE(n_out, "rz_openings_enumerate: null n_out");
+    RZ_REQUIRE(cap == 0 || (own_out && enemy_out && moves_out), "rz_openings_enumerate: null output with cap = %zu", cap);
+    *n_out = 0;
+    const cudaStream_t st = 0;
+    Buffers buf;
+    // the frontier: level 0 is the initial position, black to move
+    u64 *own, *enemy;
+    uint8_t* moves;
+    size_t n = 1;
+    RZ_TRY(buf.get(&own, 1));
+    RZ_TRY(buf.get(&enemy, 1));
+    RZ_TRY(buf.get(&moves, (size_t)plies));
+    const u64 start[2] = {kStartBlack, kStartWhite};
+    RZ_CUDA_TRY(cudaMemcpyAsync(own, &start[0], sizeof(u64), cudaMemcpyHostToDevice, st));
+    RZ_CUDA_TRY(cudaMemcpyAsync(enemy, &start[1], sizeof(u64), cudaMemcpyHostToDevice, st));
+    if (level_counts) level_counts[0] = 1;
+    for (int level = 0; level < plies; ++level) {
+        uint64_t *count, *offset;
+        RZ_TRY(buf.get(&count, n + 1));
+        RZ_TRY(buf.get(&offset, n + 1));
+        count_kernel<<<blocks_for(n), kThreads, 0, st>>>(own, enemy, n, count);
+        RZ_LAUNCH_CHECK();
+        RZ_CUDA_TRY(cudaMemsetAsync(count + n, 0, sizeof(uint64_t), st));
+        size_t tmp_bytes = 0;
+        RZ_CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, count, offset, (int64_t)(n + 1), st));
+        void* tmp;
+        RZ_TRY(buf.get((uint8_t**)&tmp, tmp_bytes));
+        RZ_CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, count, offset, (int64_t)(n + 1), st));
+        uint64_t m = 0;
+        RZ_CUDA_TRY(cudaMemcpyAsync(&m, offset + n, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+        RZ_CUDA_TRY(cudaStreamSynchronize(st));
+        buf.release(tmp);
+        buf.release(count);
+        if (m > (uint64_t)INT_MAX) {
+            set_error("rz_openings_enumerate: %llu children at ply %d exceed the sort's %d items", (unsigned long long)m, level + 1, INT_MAX);
+            return RZ_ENOMEM;
+        }
+        u64 *k_hi, *k_lo, *origin, *sorted_a, *sorted_b;
+        uint32_t *index, *index_a, *index_b;
+        RZ_TRY(buf.get(&k_hi, m));
+        RZ_TRY(buf.get(&k_lo, m));
+        RZ_TRY(buf.get(&origin, m));
+        RZ_TRY(buf.get(&index, m));
+        expand_kernel<<<blocks_for(n), kThreads, 0, st>>>(own, enemy, n, offset, k_hi, k_lo, index, origin);
+        RZ_LAUNCH_CHECK();
+        RZ_TRY(buf.get(&sorted_a, m));
+        RZ_TRY(buf.get(&sorted_b, m));
+        RZ_TRY(buf.get(&index_a, m));
+        RZ_TRY(buf.get(&index_b, m));
+        // low word first, then high word: radix sort is stable, so this orders by (hi, lo) and keeps child order in a class
+        tmp_bytes = 0;
+        RZ_CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, k_lo, sorted_a, index, index_a, (int)m, 0, 64, st));
+        RZ_TRY(buf.get((uint8_t**)&tmp, tmp_bytes));
+        RZ_CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, k_lo, sorted_a, index, index_a, (int)m, 0, 64, st));
+        gather_kernel<<<blocks_for(m), kThreads, 0, st>>>(k_hi, index_a, m, sorted_b);
+        RZ_LAUNCH_CHECK();
+        RZ_CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, sorted_b, sorted_a, index_a, index_b, (int)m, 0, 64, st));
+        buf.release(tmp);
+        uint8_t* head;
+        RZ_TRY(buf.get(&head, m));
+        head_kernel<<<blocks_for(m), kThreads, 0, st>>>(sorted_a, k_lo, index_b, m, head);
+        RZ_LAUNCH_CHECK();
+        int* n_sel;
+        RZ_TRY(buf.get(&n_sel, 1));
+        tmp_bytes = 0;
+        RZ_CUDA_TRY(cub::DeviceSelect::Flagged(nullptr, tmp_bytes, index_b, head, index_a, n_sel, (int)m, st));
+        RZ_TRY(buf.get((uint8_t**)&tmp, tmp_bytes));
+        RZ_CUDA_TRY(cub::DeviceSelect::Flagged(tmp, tmp_bytes, index_b, head, index_a, n_sel, (int)m, st));
+        int n_next = 0;
+        RZ_CUDA_TRY(cudaMemcpyAsync(&n_next, n_sel, sizeof(int), cudaMemcpyDeviceToHost, st));
+        RZ_CUDA_TRY(cudaStreamSynchronize(st));
+        for (void* p : {(void*)tmp, (void*)head, (void*)n_sel, (void*)k_hi, (void*)sorted_a, (void*)sorted_b, (void*)index,
+                        (void*)index_b, (void*)offset})
+            buf.release(p);
+        u64 *own2, *enemy2;
+        uint8_t* moves2;
+        RZ_TRY(buf.get(&own2, (size_t)n_next));
+        RZ_TRY(buf.get(&enemy2, (size_t)n_next));
+        RZ_TRY(buf.get(&moves2, (size_t)n_next * plies));
+        next_kernel<<<blocks_for((size_t)n_next), kThreads, 0, st>>>(own, enemy, moves, level, plies, index_a, origin, (size_t)n_next,
+                                                                     own2, enemy2, moves2);
+        RZ_LAUNCH_CHECK();
+        RZ_CUDA_TRY(cudaStreamSynchronize(st));
+        for (void* p : {(void*)own, (void*)enemy, (void*)moves, (void*)index_a, (void*)origin, (void*)k_lo}) buf.release(p);
+        own = own2; enemy = enemy2; moves = moves2;
+        n = (size_t)n_next;
+        if (level_counts) level_counts[level + 1] = n;
+    }
+    *n_out = n;
+    if (cap == 0) return RZ_OK;
+    if (cap < n) {
+        set_error("rz_openings_enumerate: %zu openings of %d plies, room for %zu", n, plies, cap);
+        return RZ_ECAPACITY;
+    }
+    RZ_CUDA_TRY(cudaMemcpy(own_out, own, n * sizeof(u64), cudaMemcpyDeviceToHost));
+    RZ_CUDA_TRY(cudaMemcpy(enemy_out, enemy, n * sizeof(u64), cudaMemcpyDeviceToHost));
+    RZ_CUDA_TRY(cudaMemcpy(moves_out, moves, n * (size_t)plies, cudaMemcpyDeviceToHost));
+    return RZ_OK;
+}

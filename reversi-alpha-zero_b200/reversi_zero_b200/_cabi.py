@@ -51,7 +51,7 @@ class Game(C.Structure):
     _fields_ = [("game_id", C.c_uint64), ("black", C.c_uint64), ("white", C.c_uint64), ("first_ply", C.c_int32),
                 ("n_plies", C.c_int32), ("expansions", C.c_int32), ("simulations", C.c_int32), ("winner", C.c_uint8),
                 ("black_z", C.c_int8), ("resign_enabled", C.c_uint8), ("resigned_mask", C.c_uint8), ("turn", C.c_uint8),
-                ("black_net", C.c_uint8), ("white_net", C.c_uint8), ("pad", C.c_uint8), ("table_nodes", C.c_int32), ("pad2", C.c_int32)]
+                ("black_net", C.c_uint8), ("white_net", C.c_uint8), ("opening_plies", C.c_uint8), ("table_nodes", C.c_int32), ("pad2", C.c_int32)]
 
 
 class PlayRow(C.Structure):
@@ -102,6 +102,7 @@ SIGNATURES = {
     "rz_solve_deep_table": (C.c_int, [C.c_int64]),
     "rz_solve_deep_clear": (C.c_int, []),
     "rz_solve_deep_table_stats": (C.c_int, [C.POINTER(DeepTableStats)]),
+    "rz_openings_enumerate": (C.c_int, [C.c_int, u64p, u64p, u8p, sz, C.POINTER(sz), u64p]),
     "rz_find_correct_moves_host": (C.c_uint64, [C.c_uint64, C.c_uint64]),
     "rz_calc_flip_host": (C.c_uint64, [C.c_int, C.c_uint64, C.c_uint64]),
     "rz_dihedral_host": (C.c_uint64, [C.c_uint64, C.c_int]),
@@ -132,6 +133,7 @@ SIGNATURES = {
     "rz_engine_set_max_games": (C.c_int, [vp, C.c_uint64]),
     "rz_engine_set_second_net": (C.c_int, [vp, vp, C.c_int]),
     "rz_engine_set_nets": (C.c_int, [vp, C.POINTER(vp), f32p, C.c_int, u8p, u8p, C.c_uint64]),
+    "rz_engine_set_openings": (C.c_int, [vp, u8p, u8p, C.c_uint64]),
     "rz_engine_set_resign_threshold": (C.c_int, [vp, C.c_int, C.c_float]),
     "rz_engine_search_root": (C.c_int, [vp, C.c_uint64, C.c_uint64, C.c_int, C.c_int, C.c_int, i32p, f32p]),
     "rz_engine_search_roots": (C.c_int, [vp, u64p, u64p, u8p, C.c_int, C.c_int, i32p, f32p]),

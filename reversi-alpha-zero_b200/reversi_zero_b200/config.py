@@ -147,6 +147,20 @@ class LeagueConfig(_Section):
         self.game_num_per_pair = 100
         self.play_config = None     # overrides of the evaluation play configuration
         self.anchor = 0             # index of the model whose rating is fixed at 0
+        self.openings = None        # an opening suite (path relative to the project directory): each pair of rounds starts
+                                    # from the next opening, once with each colour; None = the initial position
+
+
+class OpeningsConfig(_Section):
+    """Balanced opening suites for matches and leagues (`openings` command, lib/openings.py)"""
+
+    def __init__(self):
+        self.plies = 8
+        self.count = 500
+        self.max_abs_value = 0.2    # keep openings whose value (the network's value head, mover's view) is within this of 0
+        self.seed = None            # None = b200.seed
+        self.model = None           # blob path relative to the project directory (shape: the model section); None = best model
+        self.path = os.path.join("data", "openings", "openings.txt")  # relative to the project directory
 
 
 class Config(_Section):
@@ -161,6 +175,7 @@ class Config(_Section):
         self.nboard = NBoardConfig()
         self.b200 = B200Config()
         self.league = LeagueConfig()
+        self.openings = OpeningsConfig()
 
 
 def create_config(d=None, project_dir=None, data_dir=None):

@@ -7,6 +7,7 @@ import numpy as np
 from . import _cabi
 
 EVAL_NET, EVAL_FAKE = 0, 1
+MAX_OPENING_PLIES = 20  # RZ_MAX_OPENING_PLIES
 
 
 def engine_cfg_from_play_config(pc, pdc=None, games=1024, seed=0, eval_mode=EVAL_NET, net_impl=0, first_game_id=0,
@@ -88,7 +89,8 @@ class Engine:
                 out.append(dict(game_id=int(g.game_id), black=int(g.black), white=int(g.white), winner=int(g.winner),
                                 black_z=int(g.black_z), expansions=int(g.expansions), simulations=int(g.simulations),
                                 resign_enabled=bool(g.resign_enabled), resigned_mask=int(g.resigned_mask), turn=int(g.turn),
-                                black_net=int(g.black_net), white_net=int(g.white_net), table_nodes=int(g.table_nodes), plies=pl))
+                                black_net=int(g.black_net), white_net=int(g.white_net), opening_plies=int(g.opening_plies),
+                                table_nodes=int(g.table_nodes), plies=pl))
         return out
 
     def stats(self):
@@ -140,6 +142,22 @@ class Engine:
         _cabi.check(_cabi.lib().rz_engine_set_nets(self._h, handles, scales, len(nets), black.ctypes.data_as(_cabi.u8p),
                                                     white.ctypes.data_as(_cabi.u8p), int(black.size)), "rz_engine_set_nets")
         self.nets = list(nets)  # keep alive
+
+    def set_openings(self, openings):
+        """games from openings (rz_engine_set_openings): the game with local index i starts after the squares openings[i]
+        (a sequence of 0..RZ_MAX_OPENING_PLIES moves, 0..63), played without a search and not recorded.  Call before the
+        first run, with max_games in 1..len(openings)."""
+        n = len(openings)
+        moves = np.zeros((max(n, 1), MAX_OPENING_PLIES), np.uint8)
+        n_moves = np.zeros(max(n, 1), np.uint8)
+        for i, seq in enumerate(openings):
+            seq = [int(a) for a in seq]
+            if len(seq) > MAX_OPENING_PLIES or any(not 0 <= a < 64 for a in seq):
+                raise ValueError(f"opening {i}: {seq} is not a sequence of at most {MAX_OPENING_PLIES} squares 0..63")
+            moves[i, :len(seq)] = seq
+            n_moves[i] = len(seq)
+        _cabi.check(_cabi.lib().rz_engine_set_openings(self._h, moves.ctypes.data_as(_cabi.u8p), n_moves.ctypes.data_as(_cabi.u8p), n),
+                    "rz_engine_set_openings")
 
     def set_resign_threshold(self, threshold):
         _cabi.check(_cabi.lib().rz_engine_set_resign_threshold(self._h, 0 if threshold is None else 1,

@@ -1,9 +1,10 @@
 """Command line of the reference (run.py + manager.py):
 
-    python -m reversi_zero_b200.run {self,opt,eval,nboard,league} [-c config.yml] [--new] [--total-step N]
+    python -m reversi_zero_b200.run {self,opt,eval,nboard,league,openings} [-c config.yml] [--new] [--total-step N]
 
 ``self`` plays games, ``opt`` trains, ``eval`` promotes, ``nboard`` speaks the NBoard protocol on stdin / stdout,
-``league`` rates saved models against each other (settings in the YAML ``league:`` section).
+``league`` rates saved models against each other (settings in the YAML ``league:`` section), ``openings`` writes a suite
+of balanced openings for ``eval`` and ``league`` (settings in the YAML ``openings:`` section).
 Files go under the project directory: ``$PROJECT_DIR``, else the current directory.  Every command logs to
 ``logs/main.log``; all but ``nboard`` also log to stderr.
 """
@@ -14,7 +15,7 @@ from .config import create_config, load_yaml
 
 logger = getLogger(__name__)
 
-CMD_LIST = ['self', 'opt', 'eval', 'nboard', 'league']
+CMD_LIST = ['self', 'opt', 'eval', 'nboard', 'league', 'openings']
 
 
 def create_parser():
@@ -81,6 +82,9 @@ def start(argv=None):
     elif args.cmd == 'league':
         from .worker import league
         return league.start(config)
+    elif args.cmd == 'openings':
+        from .lib import openings
+        return openings.start(config)
 
 
 if __name__ == "__main__":

@@ -7,7 +7,10 @@ a match run concurrently on the device (``rz_engine_set_second_net``): each sear
 network, colours alternate by game index (the reference draws them at random, :70), each player keeps its own
 statistics (``share_mtcs_info = 0``, as ``ReversiPlayer(config, model, play_config=...)`` does in :69-70).  The
 verdict follows the reference's sequential bookkeeping (:44-64) over the games in game-index order, including its
-early-stop rules -- games after the point where the reference would have stopped do not count.  Weights are exchanged as float32 blobs (``*.rzblob.npy``, DESIGN.md section 9)."""
+early-stop rules -- games after the point where the reference would have stopped do not count.  Weights are exchanged as float32 blobs (``*.rzblob.npy``, DESIGN.md section 9).
+
+With ``eval.openings: <path>`` (a suite written by the ``openings`` command, relative to the project directory) game i
+starts from opening (i div 2) mod n of the suite, so every opening is played once with each colour."""
 import hashlib
 import os
 import shutil
@@ -69,15 +72,23 @@ def _eval_field(config, name, default):
     return getattr(ev, name, default) if ev is not None else default
 
 
-def play_match(config, best_net, ng_net, game_num, device=0, seed=0, first_game_id=0):
+def match_openings(game_num, suite):
+    """the opening of each game of a match: game i plays suite[(i div 2) mod n], and colours alternate with i"""
+    return [suite[(i // 2) % len(suite)] for i in range(game_num)]
+
+
+def play_match(config, best_net, ng_net, game_num, device=0, seed=0, first_game_id=0, suite=None):
     """-> (results, games): results[i] = 1 challenger won, 0 lost, None draw (worker/evaluate.py:84-96).
     ``seed`` / ``first_game_id`` select the Philox streams (dihedral choices, move sampling) of the match: callers give
-    every match its own, so that the randomness of consecutive matches is independent like the reference's."""
+    every match its own, so that the randomness of consecutive matches is independent like the reference's.
+    ``suite``: openings (lists of squares) the games start from, as ``match_openings`` assigns them; None: none."""
     pc = eval_play_config(config)
     slots = min(game_num, getattr(getattr(config, "b200", None), "games_per_gpu", 4096))
     cfg = engine_cfg_from_play_config(pc, games=slots, seed=seed, eval_mode=EVAL_NET, max_games=game_num, first_game_id=first_game_id)
     eng = Engine(cfg, best_net, device)
     eng.set_second_net(ng_net)
+    if suite:
+        eng.set_openings(match_openings(game_num, suite))
     eng.run(finished_target=game_num)
     games = sorted(eng.poll(), key=lambda g: g["game_id"])   # game-id order == local game index order (colours alternate with it)
     eng.close()
@@ -197,12 +208,24 @@ class EvaluateWorker:
         # restarts of the worker) do not replay the same dihedral / move-sampling streams
         import zlib
         seed = int(getattr(getattr(self.config, "b200", None), "seed", 0)) ^ zlib.crc32(os.path.basename(model_dir).encode())
+        suite = self.load_openings()
         results, _ = play_match(self.config, self.best_net, ng_net, game_num, self.device, seed=seed,
-                                first_game_id=self.match_count * 2 * game_num)
+                                first_game_id=self.match_count * 2 * game_num, suite=suite)
         self.match_count += 1
         replace, winning_rate, counted = match_verdict(results, game_num, replace_rate)
         logger.debug(f"winning rate {winning_rate * 100:.1f}% after {counted} games")
         return replace
+
+    def load_openings(self):
+        """the suite of ``eval.openings`` (None without one)"""
+        path = _eval_field(self.config, "openings", None)
+        if not path:
+            return None
+        from ..lib.openings import load_suite, suite_digest
+        full = os.path.join(self.config.resource.project_dir, path)
+        suite = load_suite(full)
+        logger.info(f"eval: {len(suite)} openings from {path} (sha256 {suite_digest(full)[:16]})")
+        return suite
 
     def next_generation_dir(self):
         rc = self.config.resource

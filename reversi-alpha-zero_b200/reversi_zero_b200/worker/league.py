@@ -11,7 +11,10 @@ Settings (YAML ``league:`` section):
 * ``models``: a list of blob paths or globs relative to the project directory, or mappings
   ``{path: ..., model: {cnn_filter_num: 128, ...}}`` whose ``model`` overrides ``config.model`` for that entry.  Default:
   ``<model_dir>/promoted/*.rzblob.npy`` sorted by name (``b200.keep_promoted_models`` fills that directory);
-* ``game_num_per_pair`` (default 100), ``play_config`` (a mapping), ``anchor`` (default 0).
+* ``game_num_per_pair`` (default 100), ``play_config`` (a mapping), ``anchor`` (default 0);
+* ``openings``: a suite written by the ``openings`` command (path relative to the project directory).  Game k, in round
+  r = k div P (P pairs), starts from opening (r div 2) mod n: each pair plays every opening once with each colour, and
+  with an odd ``game_num_per_pair`` the last opening once.  Default: every game starts from the initial position.
 
 The result goes to ``logs/league_<timestamp>.json`` and a rating table to the log.
 """
@@ -70,8 +73,15 @@ def schedule(n_models, games_per_pair):
     return black, white
 
 
-def play_league(config, nets, games_per_pair, device=0, seed=0, first_game_id=0):
-    """Plays the whole round-robin in one engine.  -> one record per game, in game-id order: game_id, black and white
+def league_openings(n_models, games_per_pair, suite):
+    """the opening of each game of ``schedule(n_models, games_per_pair)``: game k, in round r = k div P, plays
+    suite[(r div 2) mod n]; colours swap between rounds 2q and 2q + 1"""
+    n_pairs = n_models * (n_models - 1) // 2
+    return [suite[(k // n_pairs // 2) % len(suite)] for k in range(n_pairs * games_per_pair)]
+
+
+def play_league(config, nets, games_per_pair, device=0, seed=0, first_game_id=0, suite=None):
+    """Plays the whole round-robin in one engine, from the openings of ``suite`` (``league_openings``) when given.  -> one record per game, in game-id order: game_id, black and white
     (model indices), winner (1 black, 2 white, 3 draw) and disc_diff (black's discs minus white's at the end)."""
     pc = league_play_config(config)
     black, white = schedule(len(nets), games_per_pair)
@@ -83,6 +93,8 @@ def play_league(config, nets, games_per_pair, device=0, seed=0, first_game_id=0)
     eng = Engine(cfg, nets[0], device)
     try:
         eng.set_nets(nets, black, white)
+        if suite:
+            eng.set_openings(league_openings(len(nets), games_per_pair, suite))
         eng.run(finished_target=total)
         games = sorted(eng.poll(), key=lambda g: g["game_id"])
     finally:
@@ -233,13 +245,21 @@ class LeagueWorker:
         if not 0 <= anchor < len(entries):
             raise ValueError(f"league.anchor = {anchor} is not an index into the {len(entries)} models")
         seed = int(getattr(getattr(self.config, "b200", None), "seed", 0))
+        suite, openings = None, None
+        suite_path = _field(self.config, "openings", None)
+        if suite_path:
+            from ..lib.openings import load_suite, suite_digest
+            full = os.path.join(rc.project_dir, suite_path)
+            suite = load_suite(full)
+            openings = dict(path=os.path.relpath(full, rc.project_dir), sha256=suite_digest(full), count=len(suite))
+            logger.info(f"league: {len(suite)} openings from {openings['path']} (sha256 {openings['sha256'][:16]})")
         nets = []
         try:
             for p, mc in entries:
                 net = Net(mc, self.device)
                 net.load_blob(np.load(p))
                 nets.append(net)
-            records = play_league(self.config, nets, games_per_pair, self.device, seed=seed)
+            records = play_league(self.config, nets, games_per_pair, self.device, seed=seed, suite=suite)
         finally:
             for net in nets:
                 net.close()
@@ -256,7 +276,7 @@ class LeagueWorker:
                                games=int(played[i].sum()), score=float(s[i].sum()), elo=float(ratings[i]), ci95=float(ci[i])))
         pc = league_play_config(self.config)
         out = dict(timestamp=datetime.now().strftime("%Y%m%d-%H%M%S.%f"), seed=seed, games_per_pair=games_per_pair,
-                   games=len(records), anchor=anchor, play_config={k: v for k, v in sorted(vars(pc).items())}, models=models,
+                   games=len(records), anchor=anchor, openings=openings, play_config={k: v for k, v in sorted(vars(pc).items())}, models=models,
                    pairs=[dict(model=i, opponent=j, **pairs[(i, j)]) for (i, j) in sorted(pairs)])
         os.makedirs(rc.log_dir, exist_ok=True)
         path = os.path.join(rc.log_dir, f"league_{out['timestamp']}.json")
