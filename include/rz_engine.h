@@ -159,6 +159,20 @@ int rz_solve_deep_table_stats(rz_deep_table_stats* out);
  * output.  Device memory grows with the level; a level that does not fit returns RZ_ENOMEM.  Synchronous. */
 int rz_openings_enumerate(int plies, uint64_t* own, uint64_t* enemy, uint8_t* moves, size_t cap, size_t* n_out,
                           uint64_t* level_counts);
+/* The opening book's graph (csrc/rz_openings.cu): every opening of 0 .. plies (1..10) plies and the moves between
+ * consecutive levels, in CSR form.  Nodes, host buffers: level by level, each level exactly rz_openings_enumerate's
+ * output for that many plies (ascending canonical key; level 0 is the initial position); own[i] / enemy[i] = the node in
+ * its representative's orientation, mover's frame; key_hi[i] / key_lo[i] (nullable) = its canonical key.  level_counts
+ * (nullable, plies + 1 entries) gives the level sizes.
+ * Edges: node i's are edge_offset[i] .. edge_offset[i + 1] - 1 (edge_offset has *n_nodes + 1 entries; nodes of the last
+ * level have none), one per legal move in ascending square order in the node's frame: edge_square = the square,
+ * edge_child = the index within the next level of the child's class, or -1 when the child is not an opening (its mover
+ * must pass, or the game is over).  cap_nodes = 0: only *n_nodes and *n_edges are set (the outputs may be NULL);
+ * cap_nodes < *n_nodes or cap_edges < *n_edges: RZ_ECAPACITY.  Repeated calls give identical output; a level that does
+ * not fit in device memory returns RZ_ENOMEM.  Synchronous. */
+int rz_openings_book_graph(int plies, uint64_t* own, uint64_t* enemy, uint64_t* key_hi, uint64_t* key_lo, size_t cap_nodes,
+                           size_t* n_nodes, uint64_t* level_counts, uint64_t* edge_offset, uint8_t* edge_square,
+                           int32_t* edge_child, size_t cap_edges, size_t* n_edges);
 
 /* Scalar host twins for the single-environment Python objects (ReversiEnv / Board used by the
  * reference's evaluate.py, nboard.py, game_model.py): same header-only code as the device kernels

@@ -1,5 +1,5 @@
-// rz_openings.cuh -- one expansion step of the opening enumerator (rz_openings.cu), __host__ __device__ so that the
-// host check (tests/support/openings_check.cu) runs the same code.
+// rz_openings.cuh -- one expansion step of the opening enumerator and the book graph's edge step (rz_openings.cu),
+// __host__ __device__ so that the host checks (tests/support/openings_check.cu, book_graph_check.cu) run the same code.
 //
 // A position is held in the mover's frame (own = the side to move).  Its children are the positions after each legal
 // move, again in the new mover's frame; a child whose side to move has no legal move (a pass, or the end of the game) is
@@ -36,6 +36,30 @@ RZ_HD void canonical(u64 own, u64 enemy, u64& k_hi, u64& k_lo) {
         const u64 o = dihedral(own, t), e = dihedral(enemy, t);
         if (o < k_hi || (o == k_hi && e < k_lo)) { k_hi = o; k_lo = e; }
     }
+}
+
+// the book graph's edges of (own, enemy) (rz_openings_book_graph): its legal moves in ascending square order, each with
+// the index of its child's class among the n_next ascending keys (next_hi, next_lo) of the next level, found by binary
+// search; -1 when the child is not an opening (its mover must pass, or the game is over).  -> the number of edges.
+RZ_HD int book_edges(u64 own, u64 enemy, const u64* next_hi, const u64* next_lo, size_t n_next, uint8_t* square,
+                     int32_t* child_index) {
+    int k = 0;
+    for (u64 m = find_correct_moves(own, enemy); m; m &= m - 1, ++k) {
+        const int sq = ctz64(m);
+        square[k] = (uint8_t)sq;
+        child_index[k] = -1;
+        u64 co, ce, hi, lo;
+        if (!child(own, enemy, sq, co, ce)) continue;
+        canonical(co, ce, hi, lo);
+        size_t a = 0, b = n_next;   // the first key >= (hi, lo)
+        while (a < b) {
+            const size_t c = (a + b) / 2;
+            if (next_hi[c] < hi || (next_hi[c] == hi && next_lo[c] < lo)) a = c + 1;
+            else b = c;
+        }
+        if (a < n_next && next_hi[a] == hi && next_lo[a] == lo) child_index[k] = (int32_t)a;
+    }
+    return k;
 }
 
 }  // namespace openings

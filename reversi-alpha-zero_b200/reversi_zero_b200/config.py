@@ -136,6 +136,8 @@ class B200Config(_Section):
         self.nboard_analyze = False  # NBoard: answer `analyze` with a retrograde analysis of the game (play_game/analysis.py)
         self.nboard_exact_hint = False  # NBoard: in solver range, `hint n` reports every move's exact value (100% lines)
         self.keep_promoted_models = False  # eval: archive every promoted blob under <model_dir>/promoted/ (worker/evaluate.py)
+        self.nboard_book = None     # NBoard: an opening book (lib/book.py; path relative to the project directory) whose moves
+                                    # `go` plays and `hint` reports inside the book; None = search every move
 
 
 class LeagueConfig(_Section):
@@ -161,6 +163,19 @@ class OpeningsConfig(_Section):
         self.seed = None            # None = b200.seed
         self.model = None           # blob path relative to the project directory (shape: the model section); None = best model
         self.path = os.path.join("data", "openings", "openings.txt")  # relative to the project directory
+        self.book = None            # an opening book (lib/book.py) of `plies` plies: each opening's value is the book's
+                                    # searched value instead of the value head; None = the value head
+
+
+class BookConfig(_Section):
+    """Opening book searched on the device (`book` command, lib/book.py)"""
+
+    def __init__(self):
+        self.plies = 8
+        self.simulation_num_per_move = 400  # simulations of every leaf search
+        self.seed = None            # None = b200.seed
+        self.model = None           # blob path relative to the project directory (shape: the model section); None = best model
+        self.path = os.path.join("data", "book", "book.npz")  # relative to the project directory
 
 
 class Config(_Section):
@@ -176,6 +191,7 @@ class Config(_Section):
         self.b200 = B200Config()
         self.league = LeagueConfig()
         self.openings = OpeningsConfig()
+        self.book = BookConfig()
 
 
 def create_config(d=None, project_dir=None, data_dir=None):

@@ -8,7 +8,9 @@ head from the mover's view, lies within ``max_abs_value`` of 0, and draws ``coun
 
 Settings (YAML ``openings:`` section): ``plies`` (8), ``count`` (500), ``max_abs_value`` (0.2), ``seed`` (default
 ``b200.seed``), ``model`` (a blob path relative to the project directory, with the ``model`` section's shape; default
-the best model's blob) and ``path`` (``data/openings/openings.txt``, relative to the project directory).
+the best model's blob), ``path`` (``data/openings/openings.txt``, relative to the project directory) and ``book`` (an
+opening book of ``plies`` plies, lib/book.py, whose searched values score the openings instead of the value head; default
+none).
 """
 import ctypes as C
 import hashlib
@@ -93,6 +95,26 @@ def balanced_suite(net, plies, count, max_abs_value, seed, batch=65536):
             net.predict_dev(own_t, enemy_t, policy_t, value_t, e - s)
             torch.cuda.synchronize(dev)
             values[s:e] = value_t.cpu().numpy()
+    return select_balanced(ops, values, count, max_abs_value, seed)
+
+
+def book_suite(book, plies, count, max_abs_value, seed):
+    """balanced_suite with each opening's value taken from `book` (a lib.book.Book of `plies` plies: its searched leaf
+    values) instead of a value head.  Refuses a book of another depth."""
+    if book.plies != int(plies):
+        raise ValueError(f"{book.path or 'the book'}: a book of {book.plies} plies cannot score openings of {plies} plies")
+    ops = enumerate_openings(plies)
+    a, b = int(book.first[plies]), int(book.first[plies + 1])
+    if b - a != ops.own.size or any(canonical_key(int(ops.own[i]), int(ops.enemy[i])) !=
+                                    (int(book.keys_hi[a + i]), int(book.keys_lo[a + i])) for i in (0, ops.own.size - 1)):
+        raise ValueError(f"{book.path or 'the book'}: its level {plies} is not the openings of {plies} plies")
+    return select_balanced(ops, book.level_values(plies), count, max_abs_value, seed)
+
+
+def select_balanced(ops, values, count, max_abs_value, seed):
+    """the openings of `ops` (enumerate_openings) whose value satisfies |v| <= max_abs_value, ordered by a hash of
+    (seed, canonical key); the first `count` of them -> [SuiteEntry]"""
+    n, plies = ops.own.size, ops.moves.shape[1]
     kept = np.nonzero(np.abs(values) <= max_abs_value)[0]
     kept = sorted(kept, key=lambda i: _order_digest(seed, ops.own[i], ops.enemy[i]))[:count]
     if len(kept) < count:
@@ -170,13 +192,20 @@ def start(config, device=0):
     model = _field(config, "model", None)
     blob = os.path.join(rc.project_dir, model) if model else blob_path_of(config)
     path = os.path.join(rc.project_dir, _field(config, "path", os.path.join("data", "openings", "openings.txt")))
-    net = Net(config.model, device)
-    try:
-        net.load_blob(np.load(blob))
-        suite = balanced_suite(net, plies, count, max_abs_value, seed)
-    finally:
-        net.close()
-    save_suite(path, suite, header=[f"{len(suite)} openings of {plies} plies, |value| <= {max_abs_value}, seed {seed}",
-                                    f"model {os.path.relpath(blob, rc.project_dir)}"])
+    book_path = _field(config, "book", None)
+    if book_path:
+        from .book import load_book
+        book = load_book(os.path.join(rc.project_dir, book_path))
+        suite = book_suite(book, plies, count, max_abs_value, seed)
+        source = f"book {book_path} ({book.meta.get('simulation_num_per_move')} simulations per position)"
+    else:
+        net = Net(config.model, device)
+        try:
+            net.load_blob(np.load(blob))
+            suite = balanced_suite(net, plies, count, max_abs_value, seed)
+        finally:
+            net.close()
+        source = f"model {os.path.relpath(blob, rc.project_dir)}"
+    save_suite(path, suite, header=[f"{len(suite)} openings of {plies} plies, |value| <= {max_abs_value}, seed {seed}", source])
     logger.info(f"openings: {len(suite)} openings of {plies} plies written to {path}")
     return path

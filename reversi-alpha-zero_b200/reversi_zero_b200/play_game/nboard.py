@@ -10,19 +10,27 @@ of ``hint_callback_per_sim`` simulations ends.  With ``b200.nboard_analyze`` on,
 analysis of the game (play_game/analysis.py), which a ``ping`` interrupts as well.  With ``b200.nboard_exact_hint`` on,
 ``hint n`` in a position the player would solve reports the exact value of the best n moves (``100%`` lines, after
 ``100%W`` lines for moves whose sign is proven first); a ``ping`` interrupts it within one slice of the deep solver.
+With ``b200.nboard_book`` set to an opening book (lib/book.py) of the loaded model, ``go`` plays the book move and ``hint
+n`` reports the best n book moves, without a search, in every interior node of the book reached from the initial
+position without a pass; everywhere else they search as without a book.
 """
 import ctypes as C
+import os
 import re
 import sys
 from collections import namedtuple
 from logging import getLogger, StreamHandler, FileHandler
 from time import time
 
+import numpy as np
+
+from ..agent.model import blob_digest
 from ..agent.player import ReversiPlayer, CallbackInMCTS, solver_max_empties, solves_exactly
 from ..env.reversi_env import ReversiEnv, Player
+from ..lib.book import best_move, load_book
 from ..lib.ggf import parse_ggf, convert_to_bitboard_and_actions, convert_move_to_action, convert_action_to_move
 from ..lib.nonblocking_stream_reader import NonBlockingStreamReader
-from .common import load_model
+from .common import load_model, model_source_path
 
 logger = getLogger(__name__)
 
@@ -31,6 +39,7 @@ GoResponse = namedtuple("GoResponse", "action eval time")
 HintResponse = namedtuple("HintResponse", "action value visit")
 ExactHint = namedtuple("ExactHint", "action value depth")   # depth: "100%" exact, "100%W" win/loss proven
 HINT_TIMEOUT = 30   # the reference solver's timeout (ReversiSolver.solve)
+START_BLACK, START_WHITE = (0x10 << 24) | (0x08 << 32), (0x08 << 24) | (0x10 << 32)
 
 
 def start(config):
@@ -52,6 +61,7 @@ class NBoardEngine:
     # the same reason
     hint_solver = None
     hint_stop = None
+    book = None   # lib.book.Book of b200.nboard_book, None without a usable one
 
     def __init__(self, config, stdin=None, stdout=None):
         self.config = config
@@ -64,9 +74,40 @@ class NBoardEngine:
         self.model = load_model(self.config)
         self.play_config = self.config.play
         self.player = self.create_player()
+        self.book = self.load_book()
         self.turn_of_nboard = None
         self.game_start = None      # (black, white, player) of `set game`, and the actions since: the game `analyze` analyses
         self.game_actions = []
+
+    def load_book(self):
+        """the book of b200.nboard_book (relative to the project directory); None, logged, when none is set, the file is
+        missing or refused, or the book was searched with another model than the one loaded"""
+        path = getattr(getattr(self.config, "b200", None), "nboard_book", None)
+        if not path:
+            return None
+        full = os.path.join(self.config.resource.project_dir, path)
+        try:
+            book = load_book(full)
+        except (OSError, ValueError) as e:
+            logger.warning(f"nboard: book not used: {e}")
+            return None
+        digest = blob_digest(np.load(model_source_path(self.config)))
+        if book.meta.get("model_sha256") != digest:
+            logger.warning(f"nboard: book not used: {full} was searched with model {str(book.meta.get('model_sha256'))[:16]}, "
+                           f"the loaded model is {digest[:16]}")
+            return None
+        logger.info(f"nboard: book {full}: {book.plies} plies, {book.values.size} positions")
+        return book
+
+    def book_moves(self, own, enemy):
+        """Book.moves of the position, in a game from the initial position without a pass; else None"""
+        if self.book is None or None in self.game_actions:
+            return None
+        if self.game_start is not None:
+            black, white, player = self.game_start
+            if (black, white, int(getattr(player, "value", player))) != (START_BLACK, START_WHITE, 1):
+                return None
+        return self.book.moves(own, enemy)
 
     def create_player(self):
         logger.debug("create new ReversiPlayer()")
@@ -154,12 +195,21 @@ class NBoardEngine:
             return GoResponse(None, 0, 0)
         states = self._states()
         start_time = time()
+        book = self.book_moves(*states)
+        if book:
+            action, value = best_move(book)
+            logger.debug(f"book move {convert_action_to_move(action)} ({value:+.4f})")
+            return GoResponse(action, value, time() - start_time)
         action = self.player.action(*states)
         item = self.player.ask_thought_about(*states)
         return GoResponse(action, item.values[action], time() - start_time)
 
     def hint(self, n_hint):
         states = self._states()
+        book = self.book_moves(*states)
+        if book:
+            self.handler.report_hint(book_hints(book, n_hint, self.book.meta.get("simulation_num_per_move", 0)))
+            return
         exact = getattr(getattr(self.config, "b200", None), "nboard_exact_hint", False) and \
             solves_exactly(self.play_config, *states, solver_max_empties(self.config))
         if exact and self.exact_hint(*states, n_hint):
@@ -216,6 +266,13 @@ class NBoardEngine:
             return
         black, white, player = self.game_start
         self.analyser.analyse(black, white, player, self.game_actions, report)
+
+
+def book_hints(moves, n_hint, visits):
+    """the best `n_hint` book moves, best first as the search hint's list is (report_hint puts the best last), each with
+    the book's simulation count in the search hint's visit field"""
+    ranked = sorted(moves, key=lambda m: (-m[1], m[0]))[:n_hint]
+    return [HintResponse(sq, value, visits) for sq, value in ranked]
 
 
 def _best_last(hints):

@@ -1,10 +1,11 @@
 """Command line of the reference (run.py + manager.py):
 
-    python -m reversi_zero_b200.run {self,opt,eval,nboard,league,openings} [-c config.yml] [--new] [--total-step N]
+    python -m reversi_zero_b200.run {self,opt,eval,nboard,league,openings,book} [-c config.yml] [--new] [--total-step N]
 
 ``self`` plays games, ``opt`` trains, ``eval`` promotes, ``nboard`` speaks the NBoard protocol on stdin / stdout,
 ``league`` rates saved models against each other (settings in the YAML ``league:`` section), ``openings`` writes a suite
-of balanced openings for ``eval`` and ``league`` (settings in the YAML ``openings:`` section).
+of balanced openings for ``eval`` and ``league`` (settings in the YAML ``openings:`` section), ``book`` builds an opening
+book for NBoard and for suites (settings in the YAML ``book:`` section).
 Files go under the project directory: ``$PROJECT_DIR``, else the current directory.  Every command logs to
 ``logs/main.log``; all but ``nboard`` also log to stderr.
 """
@@ -15,7 +16,7 @@ from .config import create_config, load_yaml
 
 logger = getLogger(__name__)
 
-CMD_LIST = ['self', 'opt', 'eval', 'nboard', 'league', 'openings']
+CMD_LIST = ['self', 'opt', 'eval', 'nboard', 'league', 'openings', 'book']
 
 
 def create_parser():
@@ -85,6 +86,9 @@ def start(argv=None):
     elif args.cmd == 'openings':
         from .lib import openings
         return openings.start(config)
+    elif args.cmd == 'book':
+        from .lib import book
+        return book.start(config)
 
 
 if __name__ == "__main__":
