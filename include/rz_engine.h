@@ -173,6 +173,19 @@ int rz_openings_enumerate(int plies, uint64_t* own, uint64_t* enemy, uint8_t* mo
 int rz_openings_book_graph(int plies, uint64_t* own, uint64_t* enemy, uint64_t* key_hi, uint64_t* key_lo, size_t cap_nodes,
                            size_t* n_nodes, uint64_t* level_counts, uint64_t* edge_offset, uint8_t* edge_square,
                            int32_t* edge_child, size_t cap_edges, size_t* n_edges);
+/* The children of any n book nodes (csrc/rz_openings.cu): how an opening book grows beyond its full width and links a
+ * level that rz_openings_book_graph did not build.  Inputs, host buffers: own[i] / enemy[i] = node i in the mover's frame;
+ * next_hi / next_lo (NULL when n_next = 0) = the n_next ascending canonical keys of a sorted level.  Output, host buffers:
+ * node i's children are edge_offset[i] .. edge_offset[i + 1] - 1 (edge_offset has n + 1 entries), one per legal move in
+ * ascending square order: edge_square = the square; child_own / child_enemy = the child in the new mover's frame;
+ * child_hi / child_lo = its canonical key; child_kind = 0 kept (an opening), 1 its mover must pass, 2 the game is over;
+ * edge_child = the index of its key among next_hi / next_lo, or -1 when the child is not kept or not in that level.
+ * edge_offset = NULL: only *n_edges is set (the other outputs may be NULL too); cap_edges < *n_edges: RZ_ECAPACITY.
+ * Repeated calls give identical output.  Synchronous. */
+int rz_openings_book_children(const uint64_t* own, const uint64_t* enemy, size_t n, const uint64_t* next_hi,
+                              const uint64_t* next_lo, size_t n_next, uint64_t* edge_offset, uint8_t* edge_square,
+                              int32_t* edge_child, uint64_t* child_own, uint64_t* child_enemy, uint64_t* child_hi,
+                              uint64_t* child_lo, uint8_t* child_kind, size_t cap_edges, size_t* n_edges);
 
 /* Scalar host twins for the single-environment Python objects (ReversiEnv / Board used by the
  * reference's evaluate.py, nboard.py, game_model.py): same header-only code as the device kernels

@@ -1,4 +1,5 @@
-// rz_openings.cu -- every distinct opening of p plies, enumerated on the device (rz_openings_enumerate).
+// rz_openings.cu -- every distinct opening of p plies, enumerated on the device (rz_openings_enumerate); the opening
+// book's graph over them (rz_openings_book_graph) and the children of any list of book nodes (rz_openings_book_children).
 //
 // Level by level from the initial position: each frontier position is expanded to its children (rz_openings.cuh), the
 // children are sorted by their canonical key (two stable CUB radix sorts, low word then high word, so that equal keys
@@ -101,6 +102,20 @@ __global__ void __launch_bounds__(kThreads) edge_kernel(const u64* __restrict__ 
     const size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x;
     if (i >= n) return;
     book_edges(own[i], enemy[i], next_hi, next_lo, n_next, square + offset[i], child_index + offset[i]);
+}
+
+// the children of n nodes at their CSR offsets, against a sorted level's n_next keys
+__global__ void __launch_bounds__(kThreads) children_kernel(const u64* __restrict__ own, const u64* __restrict__ enemy, size_t n,
+                                                            const uint64_t* __restrict__ offset, const u64* __restrict__ next_hi,
+                                                            const u64* __restrict__ next_lo, size_t n_next,
+                                                            uint8_t* __restrict__ square, int32_t* __restrict__ child_index,
+                                                            u64* __restrict__ c_own, u64* __restrict__ c_enemy, u64* __restrict__ c_hi,
+                                                            u64* __restrict__ c_lo, uint8_t* __restrict__ kind) {
+    const size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x;
+    if (i >= n) return;
+    const size_t o = offset[i];
+    book_children(own[i], enemy[i], next_hi, next_lo, n_next, square + o, child_index + o, c_own + o, c_enemy + o, c_hi + o,
+                  c_lo + o, kind + o);
 }
 
 // device buffers of one call, freed on every return
@@ -336,5 +351,80 @@ extern "C" int rz_openings_book_graph(int plies, uint64_t* own_out, uint64_t* en
     RZ_CUDA_TRY(cudaMemcpy(edge_offset, offset, (n + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost));
     RZ_CUDA_TRY(cudaMemcpy(edge_square, square, (size_t)m, cudaMemcpyDeviceToHost));
     RZ_CUDA_TRY(cudaMemcpy(edge_child, child_index, (size_t)m * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    return RZ_OK;
+}
+
+// The children of any n nodes: the nodes and the level's keys copied to the device, the legal-move counts, an exclusive
+// scan of them (the CSR offsets), and the children kernel, one node per thread.
+extern "C" int rz_openings_book_children(const uint64_t* own_in, const uint64_t* enemy_in, size_t n, const uint64_t* next_hi_in,
+                                         const uint64_t* next_lo_in, size_t n_next, uint64_t* edge_offset, uint8_t* edge_square,
+                                         int32_t* edge_child, uint64_t* child_own, uint64_t* child_enemy, uint64_t* child_hi,
+                                         uint64_t* child_lo, uint8_t* child_kind, size_t cap_edges, size_t* n_edges) {
+    RZ_REQUIRE(n_edges, "rz_openings_book_children: null n_edges");
+    RZ_REQUIRE(n == 0 || (own_in && enemy_in), "rz_openings_book_children: null nodes with n = %zu", n);
+    RZ_REQUIRE(n_next == 0 || (next_hi_in && next_lo_in), "rz_openings_book_children: null keys with n_next = %zu", n_next);
+    RZ_REQUIRE(!edge_offset || (edge_square && edge_child && child_own && child_enemy && child_hi && child_lo && child_kind),
+               "rz_openings_book_children: edge_offset without the other outputs");
+    *n_edges = 0;
+    if (n == 0) {
+        if (edge_offset) edge_offset[0] = 0;
+        return RZ_OK;
+    }
+    const cudaStream_t st = 0;
+    Buffers buf("rz_openings_book_children");
+    u64 *own, *enemy, *next_hi, *next_lo;
+    uint64_t *count, *offset;
+    RZ_TRY(buf.get(&own, n));
+    RZ_TRY(buf.get(&enemy, n));
+    RZ_TRY(buf.get(&next_hi, n_next));
+    RZ_TRY(buf.get(&next_lo, n_next));
+    RZ_TRY(buf.get(&count, n + 1));
+    RZ_TRY(buf.get(&offset, n + 1));
+    RZ_CUDA_TRY(cudaMemcpyAsync(own, own_in, n * sizeof(u64), cudaMemcpyHostToDevice, st));
+    RZ_CUDA_TRY(cudaMemcpyAsync(enemy, enemy_in, n * sizeof(u64), cudaMemcpyHostToDevice, st));
+    if (n_next) {
+        RZ_CUDA_TRY(cudaMemcpyAsync(next_hi, next_hi_in, n_next * sizeof(u64), cudaMemcpyHostToDevice, st));
+        RZ_CUDA_TRY(cudaMemcpyAsync(next_lo, next_lo_in, n_next * sizeof(u64), cudaMemcpyHostToDevice, st));
+    }
+    legal_count_kernel<<<blocks_for(n), kThreads, 0, st>>>(own, enemy, n, count);
+    RZ_LAUNCH_CHECK();
+    RZ_CUDA_TRY(cudaMemsetAsync(count + n, 0, sizeof(uint64_t), st));
+    size_t tmp_bytes = 0;
+    RZ_CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, count, offset, (int64_t)(n + 1), st));
+    uint8_t* tmp;
+    RZ_TRY(buf.get(&tmp, tmp_bytes));
+    RZ_CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, count, offset, (int64_t)(n + 1), st));
+    uint64_t m = 0;
+    RZ_CUDA_TRY(cudaMemcpyAsync(&m, offset + n, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+    RZ_CUDA_TRY(cudaStreamSynchronize(st));
+    *n_edges = (size_t)m;
+    if (!edge_offset) return RZ_OK;
+    if (cap_edges < m) {
+        set_error("rz_openings_book_children: %llu children of %zu nodes, room for %zu", (unsigned long long)m, n, cap_edges);
+        return RZ_ECAPACITY;
+    }
+    buf.release(tmp);
+    buf.release(count);
+    uint8_t *square, *kind;
+    int32_t* child_index;
+    u64 *c_own, *c_enemy, *c_hi, *c_lo;
+    RZ_TRY(buf.get(&square, m));
+    RZ_TRY(buf.get(&kind, m));
+    RZ_TRY(buf.get(&child_index, m));
+    RZ_TRY(buf.get(&c_own, m));
+    RZ_TRY(buf.get(&c_enemy, m));
+    RZ_TRY(buf.get(&c_hi, m));
+    RZ_TRY(buf.get(&c_lo, m));
+    children_kernel<<<blocks_for(n), kThreads, 0, st>>>(own, enemy, n, offset, next_hi, next_lo, n_next, square, child_index, c_own,
+                                                        c_enemy, c_hi, c_lo, kind);
+    RZ_LAUNCH_CHECK();
+    RZ_CUDA_TRY(cudaMemcpy(edge_offset, offset, (n + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+    RZ_CUDA_TRY(cudaMemcpy(edge_square, square, (size_t)m, cudaMemcpyDeviceToHost));
+    RZ_CUDA_TRY(cudaMemcpy(edge_child, child_index, (size_t)m * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    RZ_CUDA_TRY(cudaMemcpy(child_own, c_own, (size_t)m * sizeof(u64), cudaMemcpyDeviceToHost));
+    RZ_CUDA_TRY(cudaMemcpy(child_enemy, c_enemy, (size_t)m * sizeof(u64), cudaMemcpyDeviceToHost));
+    RZ_CUDA_TRY(cudaMemcpy(child_hi, c_hi, (size_t)m * sizeof(u64), cudaMemcpyDeviceToHost));
+    RZ_CUDA_TRY(cudaMemcpy(child_lo, c_lo, (size_t)m * sizeof(u64), cudaMemcpyDeviceToHost));
+    RZ_CUDA_TRY(cudaMemcpy(child_kind, kind, (size_t)m, cudaMemcpyDeviceToHost));
     return RZ_OK;
 }

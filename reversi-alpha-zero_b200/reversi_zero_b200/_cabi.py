@@ -104,6 +104,8 @@ SIGNATURES = {
     "rz_solve_deep_table_stats": (C.c_int, [C.POINTER(DeepTableStats)]),
     "rz_openings_enumerate": (C.c_int, [C.c_int, u64p, u64p, u8p, sz, C.POINTER(sz), u64p]),
     "rz_openings_book_graph": (C.c_int, [C.c_int, u64p, u64p, u64p, u64p, sz, C.POINTER(sz), u64p, u64p, u8p, i32p, sz, C.POINTER(sz)]),
+    "rz_openings_book_children": (C.c_int, [u64p, u64p, sz, u64p, u64p, sz, u64p, u8p, i32p, u64p, u64p, u64p, u64p, u8p, sz,
+                                            C.POINTER(sz)]),
     "rz_find_correct_moves_host": (C.c_uint64, [C.c_uint64, C.c_uint64]),
     "rz_calc_flip_host": (C.c_uint64, [C.c_int, C.c_uint64, C.c_uint64]),
     "rz_dihedral_host": (C.c_uint64, [C.c_uint64, C.c_int]),

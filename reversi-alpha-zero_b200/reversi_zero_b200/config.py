@@ -138,6 +138,7 @@ class B200Config(_Section):
         self.keep_promoted_models = False  # eval: archive every promoted blob under <model_dir>/promoted/ (worker/evaluate.py)
         self.nboard_book = None     # NBoard: an opening book (lib/book.py; path relative to the project directory) whose moves
                                     # `go` plays and `hint` reports inside the book; None = search every move
+        self.nboard_book_learn = False  # NBoard: `learn` adds the game to the book (book: max_level) and writes it back
 
 
 class LeagueConfig(_Section):
@@ -176,6 +177,12 @@ class BookConfig(_Section):
         self.seed = None            # None = b200.seed
         self.model = None           # blob path relative to the project directory (shape: the model section); None = best model
         self.path = os.path.join("data", "book", "book.npz")  # relative to the project directory
+        self.extend = False         # grow or learn the book at `path` instead of building one (same model and simulations)
+        self.grow_nodes = 0         # best-first expansions of leaves beyond the full width; 0 = no growth
+        self.grow_batch = 256       # expansions per round (one search batch)
+        self.max_level = 40         # the deepest level growth and learning may add (at most 40: 20 empties)
+        self.grow_depth_cost = 0.0  # the priority's depth term: d + grow_depth_cost x (level - plies)
+        self.learn = None           # GGF file globs (relative to the project directory) whose games are learned
 
 
 class Config(_Section):

@@ -12,7 +12,9 @@ analysis of the game (play_game/analysis.py), which a ``ping`` interrupts as wel
 ``100%W`` lines for moves whose sign is proven first); a ``ping`` interrupts it within one slice of the deep solver.
 With ``b200.nboard_book`` set to an opening book (lib/book.py) of the loaded model, ``go`` plays the book move and ``hint
 n`` reports the best n book moves, without a search, in every interior node of the book reached from the initial
-position without a pass; everywhere else they search as without a book.
+position without a pass; everywhere else they search as without a book.  With ``b200.nboard_book_learn`` on as well,
+``learn`` adds the game since ``set game`` to the book (lib/book.learn_game, up to ``book.max_level``), writes it back to
+its file and plays from the grown book, before it replies ``learned``; a ``ping`` does not interrupt it.
 """
 import ctypes as C
 import os
@@ -27,6 +29,7 @@ import numpy as np
 from ..agent.model import blob_digest
 from ..agent.player import ReversiPlayer, CallbackInMCTS, solver_max_empties, solves_exactly
 from ..env.reversi_env import ReversiEnv, Player
+from ..lib import book as book_lib
 from ..lib.book import best_move, load_book
 from ..lib.ggf import parse_ggf, convert_to_bitboard_and_actions, convert_move_to_action, convert_action_to_move
 from ..lib.nonblocking_stream_reader import NonBlockingStreamReader
@@ -108,6 +111,31 @@ class NBoardEngine:
             if (black, white, int(getattr(player, "value", player))) != (START_BLACK, START_WHITE, 1):
                 return None
         return self.book.moves(own, enemy)
+
+    def book_searcher(self):
+        """the searcher of learned positions: the loaded model with the book's simulation count and seed"""
+        return book_lib.Searcher(self.config, self.model, self.book)
+
+    def learn(self):
+        """`learn` with b200.nboard_book_learn on and a book loaded: the game since `set game` is learned into the book,
+        which is written back to its file and used from then on.  A game the book cannot learn is logged."""
+        if self.book is None:
+            return
+        start_time = time()
+        search = self.book_searcher()
+        try:
+            max_level = int(book_lib._field(self.config, "max_level", book_lib.MAX_LEVEL))
+            book, k = book_lib.learn_game(self.book, self.game_actions, max_level, search=search, start=self.game_start)
+        except ValueError as e:
+            logger.warning(f"nboard: game not learned: {e}")
+            return
+        finally:
+            search.close()
+        if k:
+            book_lib.save_book(self.book.path, book)
+            self.book = book
+        logger.info(f"nboard: learned the game: {k} positions expanded, {self.book.values.size} positions in the book "
+                    f"({time() - start_time:.2f} s)")
 
     def create_player(self):
         logger.debug("create new ReversiPlayer()")
@@ -381,6 +409,9 @@ class NBoardProtocolVersion2:
         self.engine.reply(f"pong {n}")
 
     def learn(self):
+        """With b200.nboard_book_learn on, the engine learns the game into its book first (NBoardEngine.learn)."""
+        if getattr(getattr(self.config, "b200", None), "nboard_book_learn", False):
+            self.engine.learn()
         self.engine.reply("learned")
 
     def analyze(self):
